@@ -60,7 +60,7 @@ def parse():
     ap.add_argument("--res-blocks", type=int, default=7)
     ap.add_argument("--precision", default=os.environ.get("CCHESS_NN_PRECISION", "fp16"))
     ap.add_argument("--no-graph", action="store_true")
-    ap.add_argument("--first-conv", default=None, choices=["gather", "tc", "mma"], help="first-layer kernel: mma.sync with register-built one-hot operand (default), CUDA-core gather-add, or tcgen05/TMEM")
+    ap.add_argument("--first-conv", default=None, choices=["gather", "tc", "mma"], help="first-layer kernel: CUDA-core gather-add (default), wgmma with a shared-memory one-hot operand, or mma.sync with a register-built one")
     ap.add_argument("--lanes", type=int, default=1, choices=[1, 2], help="2 = pipeline two half-batches (tree kernel under the other half's network)")
     ap.add_argument("--library-ends", action="store_true", help="use cuDNN/cuBLAS for the first conv and the heads instead of csrc/cz_net.cu")
     ap.add_argument("--legs", default=os.environ.get("CCHESS_BENCH_LEGS", ALL_LEGS), help="comma list of extra legs (%s) or 'none'" % ALL_LEGS)
@@ -69,13 +69,14 @@ def parse():
     ap.add_argument("--soak-plies", type=int, default=170)
     ap.add_argument("--profile-waves", type=int, default=200, help="waves timed individually for the roofline line")
     ap.add_argument("--arena-words", type=int, default=0)
-    ap.add_argument("--kwave-capture", action="store_true", help="ncu helper: play --warmup plies (deep trees), then run --profile-waves eager waves and exit")
+    ap.add_argument("--kwave-capture", action="store_true", help="profiler helper: play --warmup plies (deep trees), then run --profile-waves eager waves and exit")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write what the last timed step computed to DIR/<name>.npy")
     return ap.parse_args()
 
 
 # ---------------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -124,7 +125,7 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)", d
-    return 6650.0, "fallback (B200_PROFILING.md)", {}
+    return 3350.0, "H100 SXM data sheet (HBM3)", {}
 
 
 def algorithmic_bytes(c0, c1, enc_bytes):
@@ -311,6 +312,7 @@ class Runner:
         self.barrier()
         t0 = time.perf_counter()
         ev0.record()
+        out = None
         for _ in range(steps):
             out = sp.step()
             if self.gather is not None:                         # counts of step s, payload of step s-1, landed tuples of step s-2: all asynchronous
@@ -338,7 +340,7 @@ class Runner:
         dev_ms, e2e_ms, wall_ms = [float(x) for x in t]
         tot_exp, tot_launch, games_done, tuples_done = [float(x) for x in n]
         return dict(dev_ms=dev_ms, e2e_ms=e2e_ms, wall_ms=wall_ms, expansions=tot_exp, launches=tot_launch, games_done=games_done,
-                    tuples_done=tuples_done, waves=sp.waves - waves0, steps=steps, c0=c0, c1=c1, clocks=clk,
+                    tuples_done=tuples_done, waves=sp.waves - waves0, steps=steps, c0=c0, c1=c1, clocks=clk, last=out,
                     value=tot_exp / (dev_ms * 1e-3), e2e=tot_exp / (e2e_ms * 1e-3))
 
     def kwave_roofline(self, n_waves):
@@ -547,6 +549,27 @@ def leg_soak(runner, plies):
                 note="seed-0 (untrained) network: games end by king capture or the 60-ply no-capture rule (main.py:1532-1545)")
 
 
+DUMP_ARRAY_BYTES = 16 << 20      # larger arrays are dumped as a fixed, seeded sample of rows (four such arrays stay within 64 MB)
+
+
+def dump_outputs(d, sp, out):
+    """--dump-outputs: what the last timed step handed to its caller (SelfPlay.step: chosen child per game, win rate, the status arrays
+    after the move) and the network outputs of that step's last wave (logits, value), as float32 / float64 .npy files.  Inputs are
+    seeded (seed-0 network, per-game seeds), so two builds run with the same arguments can be compared array for array."""
+    os.makedirs(d, exist_ok=True)
+    lanes = sp.lanes if sp.lanes is not None else [sp]
+    arrays = dict(choice=out["choice"], win_rate=out["win_rate"],
+                  last_wave_logits=torch.cat([ln.logits for ln in lanes]), last_wave_value=torch.cat([ln.value for ln in lanes]))
+    arrays.update(("status_" + k, v) for k, v in out["status"].items())
+    for name, v in arrays.items():
+        v = v.detach().cpu().numpy() if torch.is_tensor(v) else np.asarray(v)
+        v = v.astype(np.float32 if v.dtype in (np.float16, np.float32) else np.float64)
+        if v.nbytes > DUMP_ARRAY_BYTES and v.ndim > 0:
+            rows = DUMP_ARRAY_BYTES // max(1, v.nbytes // v.shape[0])
+            v = v[np.sort(np.random.RandomState(0).choice(v.shape[0], rows, replace=False))]
+        np.save(os.path.join(d, name + ".npy"), v)
+
+
 # ---------------------------------------------------------------------------------------------
 def run_ours(a, rank, world, local_rank):
     import torch.distributed as dist
@@ -565,6 +588,8 @@ def run_ours(a, rank, world, local_rank):
 
     clocks = ClockSampler(local_rank) if rank == 0 else None
     m = main.plies(a.steps, a.warmup, clocks=clocks)
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, sp, m["last"])
     roof = main.kwave_roofline(a.profile_waves) if rank == 0 else None
     if world > 1:
         dist.barrier()
@@ -577,7 +602,7 @@ def run_ours(a, rank, world, local_rank):
                  mean_children=(c1["sum_C"] - m["c0"]["sum_C"]) / max(1, c1["n_expand"] - m["c0"]["n_expand"]))
     _, _, peaks = measured_peaks()
     tpeak = float(peaks.get("bf16_tflops_sustained", 0) or 0)
-    # the kernels that DOMINATE a wave are the library tcgen05 convolutions of the residual tower: their share of the roofline over the
+    # the kernels that DOMINATE a wave are the library (cuDNN) convolutions of the residual tower: their share of the roofline over the
     # whole search (all other kernels, launch gaps and the tree kernel included in the time), against the measured sustained bf16 peak
     extra["tower_roofline"] = dict(bound="tensor", achieved=extra["nn_tflops"], unit="TFLOP/s", peak=tpeak or None,
                                    frac=(extra["nn_tflops"] / tpeak) if tpeak else None,
@@ -633,7 +658,7 @@ def run_ours(a, rank, world, local_rank):
                                 cuda_graph=not a.no_graph, lanes=a.lanes,
                                 fused_conv_epilogue=plan.fused,
                                 network_ends=("csrc/cz_net.cu (board-byte first conv [%s], fused heads)" % plan.first_conv) if plan.dtype == torch.uint8 else "library",
-                                l2_policy="working set (trees %.1f GB + activations) exceeds the 126 MB L2" % (c1["max_arena_words"] * 4 * B / 1e9)),
+                                l2_policy="working set (trees %.1f GB + activations) exceeds the 50 MB L2" % (c1["max_arena_words"] * 4 * B / 1e9)),
                     e2e=dict(value=m["e2e"], unit="expansions/s", h2d_bytes_per_step=h2d, d2h_bytes_per_step=d2h, wall_ms=m["wall_ms"]),
                     gpu_launches=int(m["launches"]), clocks=m["clocks"], roofline=roof, cpu_baseline=cpu, extra=extra)
         print(json.dumps(line), flush=True)

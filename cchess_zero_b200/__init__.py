@@ -1,4 +1,4 @@
-"""cchess_zero_b200 -- B200-native batched MCTS self-play engine for Chinese chess.
+"""cchess_zero_b200 -- batched MCTS self-play engine for Chinese chess on the H100 (sm_90a).
 
 Public surface mirrors the reference's Python API (chengstone/cchess-zero main.py):
 GameBoard, MCTS_tree, cchess_main, policy_value_network, plus the batched Engine / SelfPlay drivers."""

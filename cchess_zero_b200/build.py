@@ -1,4 +1,4 @@
-"""Builds libcchess_b200.so (the C-ABI engine library) in-tree with nvcc for sm_100a."""
+"""Builds libcchess_b200.so (the C-ABI engine library) in-tree with nvcc for sm_90a (H100)."""
 import os
 import subprocess
 import sys
@@ -6,10 +6,10 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = [os.path.join(HERE, "csrc", "cz_engine.cu"), os.path.join(HERE, "csrc", "cz_net.cu"), os.path.join(HERE, "csrc", "cz_tower.cu"),
        os.path.join(HERE, "csrc", "cz_host.cu")]
-DEPS = SRC + [os.path.join(HERE, "csrc", "cz_rules.cuh"), os.path.join(os.path.dirname(HERE), "include", "cchess_b200.h")]
+DEPS = SRC + [os.path.join(HERE, "csrc", "cz_rules.cuh"), os.path.join(HERE, "csrc", "cz_wgmma.cuh"), os.path.join(os.path.dirname(HERE), "include", "cchess_b200.h")]
 LIB = os.path.join(HERE, "libcchess_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "--fmad=false",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--fmad=false",
          "-Xcompiler", "-fPIC", "-Xcompiler", "-ffp-contract=off", "-shared", "-Xptxas", "-v"]
 
 

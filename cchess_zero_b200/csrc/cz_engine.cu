@@ -1,4 +1,4 @@
-// cz_engine.cu -- batched MCTS self-play engine for sm_100a (one warp per game) + its C ABI.
+// cz_engine.cu -- batched MCTS self-play engine for sm_90a (one warp per game) + its C ABI.
 //
 // Replaces, for thousands of concurrent games, the reference's leaf_node / MCTS_tree /
 // GameBoard hot path (main.py:93-206, 234-577, 579-1109) with search_threads = 1 semantics
@@ -1545,8 +1545,8 @@ static int create_engine(int n_games, int64_t arena_words, int device, int leave
     d.K = K;
     d.narr = fifo ? 6 : 5;
     {
-        int sms = 148;
-        if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || sms <= 0) sms = 148;
+        int sms = 132;
+        if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || sms <= 0) sms = 132;
         int w = (n_games + sms - 1) / sms;
         e->wpb = w < 1 ? 1 : (w > MAX_WPB ? MAX_WPB : w);
     }
@@ -1698,7 +1698,7 @@ int cz_engine_wave_compact(cz_engine *e, void *stream, void *nn_stage, void *nn_
     e->d.compact = 0;
     if (rc) return rc;
     k_compact_scan<<<1, 1024, 0, st>>>(e->d);
-    int sms = 148;
+    int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, e->device);
     k_compact_rows<<<2 * sms, 256, 0, st>>>(e->d, (const uint2 *)nn_stage, (uint2 *)nn_dense, row_bytes / 8);
     CUDA_TRY(cudaGetLastError());

@@ -1,19 +1,19 @@
-// cz_net.cu -- hand-written sm_100a kernels for the two ends of the policy-value network
+// cz_net.cu -- hand-written sm_90a kernels for the two ends of the policy-value network
 // (policy_value_network.py:45-74): the first convolution evaluated straight from board bytes, and the
-// fused policy / value heads.  The batch-1024 residual tower in between stays on the library tcgen05 path.
+// fused policy / value heads.  The batch-1024 residual tower in between stays on the library (cuDNN) path.
 //
 //   k_first_conv      : canonical board bytes -> conv3x3(14->128)+bias+ReLU output, fp16 NHWC [B][90][128].
 //                       The 14-plane input is one-hot and <= 32 of its 1260 cells are set, so the convolution is a
 //                       gather-add of weight rows: out[cell][:] = b + sum over the 3x3 neighbourhood of W[tap][piece][:].
 //                       The [9][10][14] tensor (and the reference's rank*9+file indexing, main.py:550-555) is never
 //                       materialised: image cell (r, f) reads canonical board byte r*9+f.
-//   k_first_conv_tc   : the same layer on tcgen05 + TMEM (one-hot im2col operand built in shared memory).
+//   k_first_conv_tc   : the same layer on wgmma (one-hot im2col operand built in shared memory).
 //   k_head_conv_mma   : conv1x1(128->3)+bias+ReLU (policy 2 ch + value 1 ch) as one streaming pass on mma.sync (hi+lo fp16
 //                       weight split: fp32-weight accuracy); writes the policy features hp either row-major fp16 [B][192]
-//                       (flatten order (h, w, c), zero padded) or directly as tcgen05 operand tiles.  k_head_conv: round-1 SIMT form.
+//                       (flatten order (h, w, c), zero padded) or directly as wgmma operand tiles.  k_head_conv: round-1 SIMT form.
 //   k_value_mlp       : 90 -> 256 ReLU -> 1 tanh, 8 positions per CTA, all 90 weights of a hidden unit requested up front.
-//   k_policy_fc_tc    : logits[B][2086] = hp . Wp^T + bp on tcgen05 + TMEM; both operands arrive as 48 KB bulk async copies
-//                       (cp.async.bulk) already in the UMMA layout; fp32 logits stored 128 B per warp and position.
+//   k_policy_fc_tc    : logits[B][2086] = hp . Wp^T + bp on wgmma; both operands arrive as 48 KB bulk async copies
+//                       (cp.async.bulk) already in the operand layout; fp32 logits stored 128 B per warp and position.
 //   k_policy_fc       : the same on mma.sync m16n8k16 (small batches, row-major hp).
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -22,8 +22,11 @@
 #include <string.h>
 
 #include "../../include/cchess_b200.h"
+#include "cz_wgmma.cuh"
 
 namespace {
+
+using namespace cz_sm90;
 
 // ------------------------------------------------------------------------------------------
 // first convolution from board bytes: one CTA per position, a half-warp per output cell (128 channels, 8 per lane)
@@ -78,7 +81,7 @@ __device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], 
 // first convolution on mma.sync with the ONE-HOT operand built in registers (alternative; measured 20.4 us vs 12.8 us for the gather-add
 // at 1024 positions: each warp streams the whole 36 KB of weight fragments from shared memory per 16-cell tile -- not adopted).
 //   D[16 cells][128 ch] = A[16][144] . B[144][128],  K = 9 taps x 16 piece slots (slot 0 = empty -> zero weight row; slot 15 of the
-//   centre tap is a constant 1 against the bias row, as in the tcgen05 variant).  A never exists anywhere: lane (g, t) of the warp
+//   centre tap is a constant 1 against the bias row, as in the wgmma variant).  A never exists anywhere: lane (g, t) of the warp
 //   derives its m16n8k16 fragment words for tap `tap` from the two piece codes of its rows g and g + 8 -- a 1.0 in the half that
 //   matches the code, zero otherwise (~10 ALU instructions per tap).  B is the weight matrix pre-arranged on the host in FRAGMENT
 //   order [k-step 9][n-tile 16][lane 32][2 words], copied once per CTA into shared memory: one conflict-free LDS.64 per MMA.
@@ -141,56 +144,34 @@ __global__ void __launch_bounds__(256) k_first_conv_mma(const uint8_t *__restric
 }
 
 // ------------------------------------------------------------------------------------------
-// first convolution on the 5th-generation tensor cores (tcgen05 + TMEM), one 128-cell tile per CTA.
-//   D[128 cells][128 ch] (f32, TMEM) = A[128][144] . B[144][128],  K = 9 taps x 16 "piece slots"
-//   A is ONE-HOT and never exists in global memory: thread r builds row r (its cell's 3x3 neighbourhood, one 16-wide
-//   slot per tap with a 1.0 at the piece code; code 0 = empty / off-board hits an all-zero weight row) straight into
-//   shared memory in the canonical K-major no-swizzle UMMA layout; B (the folded conv weights, same layout, prepared once
-//   on the host) is copied from L2.  One elected thread issues 9 tcgen05.mma (M128 N128 K16, kind::f16, f32 accumulate),
-//   commits to an mbarrier; the four warps read their TMEM lane quarter back with tcgen05.ld, add bias, ReLU, store fp16.
+// first convolution on the Hopper tensor cores (wgmma), one 128-cell tile per CTA iteration.
+//   D[128 cells][128 ch] (f32, registers) = A[128][144] . B[144][128],  K = 9 taps x 16 "piece slots"
+//   A is ONE-HOT and never exists in global memory: row r (its cell's 3x3 neighbourhood, one 16-wide slot per tap with a 1.0 at the
+//   piece code; code 0 = empty / off-board hits an all-zero weight row) is built straight into shared memory in the canonical
+//   K-major no-swizzle layout by two threads (taps 0-4 and 5-8); B (the folded conv weights, same layout, prepared once on the host)
+//   is copied from L2.  Two warpgroups, one per 64-row half, each issue 9 wgmma m64n128k16 (f16 in, f32 accumulate); the epilogue
+//   applies ReLU and converts to fp16 straight from the accumulator registers.
 // Shared-memory operand layout (both A and B): [k-chunk of 8 halves (18)][8-row group (16)][row in group (8)][8 halves]
 //   -> core matrix = 128 contiguous bytes, SBO (next 8-row group) = 128 B, LBO (next k-chunk) = 2048 B.
 // ------------------------------------------------------------------------------------------
 constexpr int TC_TILE_BYTES = 18 * 16 * 128;   // 36 864 B per operand
+constexpr int TC_OUT_BYTES = 128 * 256;        // fp16 output tile, staged for coalesced stores
 
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ uint64_t umma_desc_kmajor_noswizzle(uint32_t smem_addr) {
-    // cute::UMMA::SmemDescriptor (mma_sm100_desc.hpp): start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | version=1 [46,48) | layout_type=0 (no swizzle) [61,64)
-    return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | ((uint64_t)(2048u >> 4) << 16) | ((uint64_t)(128u >> 4) << 32) | (1ull << 46);
-}
-
-// Persistent: each CTA copies B and allocates TMEM once, then walks tiles blockIdx.x, +gridDim.x, ... (three CTAs per SM so that one
-// CTA's epilogue overlaps the others' operand build).  The bias rides in the GEMM: slot 15 of the centre tap is a constant 1 in A
-// and the bias row in B, so the epilogue is ReLU + fp16 convert only.
-__global__ void __launch_bounds__(128) k_first_conv_tc(const uint8_t *__restrict__ boards, int B, const uint4 *__restrict__ wB /* TC_TILE_BYTES */,
-                                                        __half *__restrict__ out /* [B][90][128] */) {
+// Persistent: each CTA copies B once, then walks tiles blockIdx.x, +gridDim.x, ... (one CTA per SM: 162 registers x 256 threads).
+// The bias rides in the GEMM: slot 15 of the centre tap is a constant 1 in A and the bias row
+// in B, so the epilogue is ReLU + fp16 convert only.
+__global__ void __launch_bounds__(256) k_first_conv_tc(const uint8_t *__restrict__ boards, int B, const uint4 *__restrict__ wB /* TC_TILE_BYTES */,
+                                                           __half *__restrict__ out /* [B][90][128] */) {
     extern __shared__ __align__(128) unsigned char smem_tc[];
-    unsigned char *sA = smem_tc, *sB = smem_tc + TC_TILE_BYTES;
-    __shared__ __align__(8) uint64_t mbar;
-    __shared__ uint32_t tmem_slot;
-    const int tid = threadIdx.x, warp = tid >> 5;
+    unsigned char *sA = smem_tc, *sB = smem_tc + TC_TILE_BYTES, *sOut = smem_tc + 2 * TC_TILE_BYTES;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
     const long long total = (long long)B * 90;
     const long long tiles = (total + 127) / 128;
 
-    if (warp == 0) {   // TMEM: 128 columns x 128 lanes of f32 accumulators
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)), "r"(128u));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-    }
-    if (tid == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(&mbar)), "r"(1u));
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    for (int i = tid; i < TC_TILE_BYTES / 16; i += 128) reinterpret_cast<uint4 *>(sB)[i] = __ldg(wB + i);   // B operand, once
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem = tmem_slot;
-    // instruction descriptor (cute::UMMA::InstrDescriptor): c_format F32 (1<<4), a/b F16 K-major, N=128 (16<<17), M=128 (8<<24)
-    const uint32_t idesc = (1u << 4) | (16u << 17) | (8u << 24);
-    const uint64_t da = umma_desc_kmajor_noswizzle(smem_u32(sA)), db = umma_desc_kmajor_noswizzle(smem_u32(sB));
-    unsigned char *rowp = sA + (tid >> 3) * 128 + (tid & 7) * 16;
-    uint32_t phase = 0;
+    for (int i = tid; i < TC_TILE_BYTES / 16; i += 256) reinterpret_cast<uint4 *>(sB)[i] = __ldg(wB + i);   // B operand, once
+    const uint64_t da = gmma_desc(smem_u32(sA) + (uint32_t)(wg * 64 * 16), 2048), db = gmma_desc(smem_u32(sB), 2048);
+    const int row = tid & 127, t_lo = wg ? 5 : 0, t_hi = wg ? 9 : 5;   // this thread builds taps [t_lo, t_hi) of A row `row`
+    unsigned char *rowp = sA + row * 16;
 
     // piece codes of the 3x3 neighbourhood of cell c (0 = empty / outside the board / beyond the batch)
     auto load_codes = [&](long long c, int (&pc)[9]) {
@@ -208,12 +189,13 @@ __global__ void __launch_bounds__(128) k_first_conv_tc(const uint8_t *__restrict
         }
     };
     int pc[9], pcn[9];
-    load_codes((long long)blockIdx.x * 128 + tid, pc);
+    load_codes((long long)blockIdx.x * 128 + row, pc);
 
     for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-        // ---- A operand: one-hot row of this thread's cell (row `tid` of the tile) ----
+        // ---- A operand: one-hot row of this thread's cell (row `row` of the tile), this thread's taps ----
 #pragma unroll
         for (int t = 0; t < 9; t++) {
+            if (t < t_lo || t >= t_hi) continue;
             const uint32_t one = 0x3C00u << ((pc[t] & 1) * 16);      // fp16 1.0 in the low or high half of a word
             const int w = pc[t] >> 1;                                  // word 0..7 inside the 16-wide slot
             uint4 lo, hi;
@@ -223,79 +205,47 @@ __global__ void __launch_bounds__(128) k_first_conv_tc(const uint8_t *__restrict
             *reinterpret_cast<uint4 *>(rowp + (2 * t) * 2048) = lo;
             *reinterpret_cast<uint4 *>(rowp + (2 * t + 1) * 2048) = hi;
         }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); // generic-proxy smem writes -> visible to the tensor core
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); // generic-proxy smem writes (A, and B on the first tile) -> visible to the tensor cores
         __syncthreads();
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        if (tid == 0) {
+        float d[64];
 #pragma unroll
-            for (int t = 0; t < 9; t++) {
-                const uint64_t a = da + (uint64_t)((t * 4096) >> 4), b = db + (uint64_t)((t * 4096) >> 4);   // two k-chunks per MMA
-                const uint32_t acc = t > 0 ? 1u : 0u;
-                asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                             "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                             ::"r"(tmem), "l"(a), "l"(b), "r"(idesc), "r"(acc) : "memory");
-            }
-            asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(&mbar)) : "memory");
-        }
-        load_codes((tile + gridDim.x) * 128 + tid, pcn);             // next tile's board bytes fly while the tensor core works
-        {   // wait for this tile's MMAs
-            const uint32_t bar = smem_u32(&mbar);
-            asm volatile("{\n\t.reg .pred p;\n\tWAIT_%=:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t@p bra DONE_%=;\n\tbra WAIT_%=;\n\tDONE_%=:\n\t}"
-                         ::"r"(bar), "r"(phase) : "memory");
-            phase ^= 1u;
-        }
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        // ---- epilogue: warp w owns TMEM lanes 32w..32w+31 = tile rows; thread = one row, 4 x 32 columns.  The fp16 row is
-        // staged in shared memory (the A tile is dead once the mbarrier fired) with an XOR swizzle on the 16-byte chunk index,
-        // then written with fully coalesced 512-byte warp stores (two rows per instruction). ----
-        unsigned char *stage = sA + warp * (32 * 256);                 // this warp's 32 rows x 256 B
-        const int lane = tid & 31;
-#pragma unroll 1
-        for (int q = 0; q < 4; q++) {
-            uint32_t v[32];
-            const uint32_t taddr = tmem + ((uint32_t)(warp * 32) << 16) + (uint32_t)(q * 32);
-            asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                         "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                         "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                         : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                           "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-                           "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-                           "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                         : "r"(taddr));
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+        for (int i = 0; i < 64; i++) d[i] = 0.f;
+        wgmma_fence();
 #pragma unroll
-            for (int j = 0; j < 4; j++) {
-                uint4 o;
-                __half2 *oh = reinterpret_cast<__half2 *>(&o);
+        for (int t = 0; t < 9; t++) Wgmma<128>::mma(d, da + (uint64_t)((t * 4096) >> 4), db + (uint64_t)((t * 4096) >> 4), 1u);   // two k-chunks per MMA
+        wgmma_commit();
+        load_codes((tile + gridDim.x) * 128 + row, pcn);             // next tile's board bytes fly while the tensor cores work
+        wgmma_wait<0>();
+        fence_regs(d);
+        // ---- epilogue: this warp owns tile rows rb .. rb+15 (lane: rows rb + lane/4 and + 8, channel pairs 8j + 2(lane%4)).  The fp16
+        // rows are staged in this warp's private slice of sOut with an XOR swizzle on the 16-byte chunk index (conflict-free), then
+        // written with fully coalesced 512-byte warp stores (two rows per instruction). ----
+        const int rb = wg * 64 + (warp & 3) * 16, q = lane & 3;
 #pragma unroll
-                for (int k = 0; k < 4; k++)
-                    oh[k] = __floats2half2_rn(fmaxf(__uint_as_float(v[j * 8 + k * 2]), 0.f), fmaxf(__uint_as_float(v[j * 8 + k * 2 + 1]), 0.f));
-                const int chunk = q * 4 + j;
-                *reinterpret_cast<uint4 *>(stage + lane * 256 + ((chunk ^ (lane & 15)) << 4)) = o;
-            }
+        for (int h = 0; h < 2; h++) {
+            const int r = rb + (lane >> 2) + 8 * h;
+#pragma unroll
+            for (int j = 0; j < 16; j++)
+                *reinterpret_cast<__half2 *>(sOut + r * 256 + ((j ^ (r & 15)) << 4) + q * 4) =
+                    __floats2half2_rn(fmaxf(d[4 * j + 2 * h], 0.f), fmaxf(d[4 * j + 2 * h + 1], 0.f));
         }
         __syncwarp();
         {
-            const long long row0 = tile * 128 + warp * 32;             // first cell of this warp's 32 rows
+            const long long row0 = tile * 128 + rb;                    // first cell of this warp's 16 rows
             const int half = lane >> 4, ch = lane & 15;
 #pragma unroll 4
-            for (int i = 0; i < 16; i++) {
+            for (int i = 0; i < 8; i++) {
                 const int r = 2 * i + half;
                 if (row0 + r < total) {
-                    const uint4 o = *reinterpret_cast<const uint4 *>(stage + r * 256 + ((ch ^ (r & 15)) << 4));
+                    const uint4 o = *reinterpret_cast<const uint4 *>(sOut + (rb + r) * 256 + ((ch ^ ((rb + r) & 15)) << 4));
                     *reinterpret_cast<uint4 *>(out + (size_t)(row0 + r) * 128 + ch * 8) = o;
                 }
             }
         }
-        // the next tile overwrites A (its MMAs are complete: mbarrier) and the accumulators (every warp must have drained its lanes)
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncthreads();
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+        __syncthreads();                                               // every warpgroup's MMAs have read A before the next tile overwrites it
 #pragma unroll
         for (int t = 0; t < 9; t++) pc[t] = pcn[t];
     }
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(128u));
 }
 
 // ------------------------------------------------------------------------------------------
@@ -400,7 +350,7 @@ __global__ void __launch_bounds__(256) k_value_mlp(const float *__restrict__ hv 
 // equals the fp32-weight dot product to ~1e-7 relative: no precision is traded for the speed.  ~2 instructions per cell.
 // ------------------------------------------------------------------------------------------
 constexpr int HC_ROW = 136;   // halves per staged row (128 + 8 pad = 272 B)
-// TILED: hp is written in the UMMA operand layout k_policy_fc_tc consumes: [position tile of 128][k-chunk 24][128 positions][8 halves].
+// TILED: hp is written in the operand layout k_policy_fc_tc consumes: [position tile of 128][k-chunk 24][128 positions][8 halves].
 template <bool TILED>
 __global__ void __launch_bounds__(192) k_head_conv_mma(const __half *__restrict__ x /* [B][90][128] */, int B, const float *__restrict__ wh /* [3][128] */,
                                                         const float *__restrict__ bh /* [3] */, __half *__restrict__ hp /* [B][192] or tiled */,
@@ -467,91 +417,81 @@ __global__ void __launch_bounds__(192) k_head_conv_mma(const __half *__restrict_
 }
 
 // ------------------------------------------------------------------------------------------
-// heads, stage 2b on the 5th-generation tensor cores: logits[pos][label] = hp[pos] . wp[label] + bp[label]   (tcgen05 + TMEM)
-//   D[128 labels][128 positions] (f32, TMEM) = A[128][192] . B[192][128]: A = a 128-label tile of the FC weights, B = a 128-position
-//   tile of the head features, both already in the canonical K-major no-swizzle UMMA layout in global memory (weights: prepared once
+// heads, stage 2b on the Hopper tensor cores: logits[pos][label] = hp[pos] . wp[label] + bp[label]   (wgmma)
+//   D[128 labels][128 positions] (f32) = A[128][192] . B[192][128]: A = a 128-label tile of the FC weights, B = a 128-position
+//   tile of the head features, both already in the canonical K-major no-swizzle layout in global memory (weights: prepared once
 //   on the host; features: written that way by k_head_conv_mma<true>), so each operand is ONE 48 KB bulk async copy
-//   (cp.async.bulk, SASS UBLKCP) signalling an mbarrier.  One elected thread issues 12 tcgen05.mma (M128 N128 K16), commits; the four
-//   warps read their TMEM lane quarter (lane = label) 32 positions at a time and store logits[pos][label0 .. label0+31] -- 128
-//   contiguous bytes per warp and position.  136 CTAs for 1024 positions x 2086 labels, one tile each.
+//   (cp.async.bulk) signalling an mbarrier.  Two warpgroups, one per 64-label half, each issue 12 wgmma m64n128k16; the tile is then
+//   staged transposed in the (dead) operand buffers so that every warp stores 128 contiguous bytes of logits per position.
+//   136 CTAs for 1024 positions x 2086 labels, one tile each.
 // ------------------------------------------------------------------------------------------
 constexpr int FC_TILE_BYTES = 24 * 128 * 16;   // 49 152 B per operand tile
-__global__ void __launch_bounds__(128) k_policy_fc_tc(const uint4 *__restrict__ hp_tiled, int B, const uint4 *__restrict__ wp_tiled,
+constexpr int FC_OUT_ROW = 132;                // floats per staged position row: 128 labels + 4 pad (conflict-free fragment stores)
+__global__ void __launch_bounds__(256) k_policy_fc_tc(const uint4 *__restrict__ hp_tiled, int B, const uint4 *__restrict__ wp_tiled,
                                                        const float *__restrict__ bp /* [>= 2176] */, float *__restrict__ logits /* [B][2086] */) {
     extern __shared__ __align__(128) unsigned char smem_fc_tc[];
     unsigned char *sA = smem_fc_tc, *sB = smem_fc_tc + FC_TILE_BYTES;
-    __shared__ __align__(8) uint64_t bar_ld, bar_mma;
-    __shared__ uint32_t tmem_slot;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    float *sOut = reinterpret_cast<float *>(smem_fc_tc);            // [128 positions][FC_OUT_ROW], once the MMAs are done
+    __shared__ __align__(8) uint64_t bar_ld;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
     const int mt = blockIdx.y, nt = blockIdx.x;                     // label tile, position tile
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)), "r"(128u));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-    }
     if (tid == 0) {
         asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(&bar_ld)), "r"(1u));
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(&bar_mma)), "r"(1u));
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem = tmem_slot;
     if (tid == 0) {
         asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(&bar_ld)), "r"(2u * FC_TILE_BYTES) : "memory");
         asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                      ::"r"(smem_u32(sA)), "l"(reinterpret_cast<const unsigned char *>(wp_tiled) + (size_t)mt * FC_TILE_BYTES), "r"(FC_TILE_BYTES), "r"(smem_u32(&bar_ld)) : "memory");
         asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                      ::"r"(smem_u32(sB)), "l"(reinterpret_cast<const unsigned char *>(hp_tiled) + (size_t)nt * FC_TILE_BYTES), "r"(FC_TILE_BYTES), "r"(smem_u32(&bar_ld)) : "memory");
-        {   // operands landed
-            const uint32_t bar = smem_u32(&bar_ld);
-            asm volatile("{\n\t.reg .pred p;\n\tWAIT_%=:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t@p bra DONE_%=;\n\tbra WAIT_%=;\n\tDONE_%=:\n\t}"
-                         ::"r"(bar), "r"(0u) : "memory");
-        }
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t idesc = (1u << 4) | (16u << 17) | (8u << 24);          // f32 accumulate, f16 x f16, N = 128, M = 128
-        const uint64_t da = umma_desc_kmajor_noswizzle(smem_u32(sA)), db = umma_desc_kmajor_noswizzle(smem_u32(sB));
-#pragma unroll
-        for (int ks = 0; ks < 12; ks++) {
-            const uint64_t a = da + (uint64_t)((ks * 4096) >> 4), b = db + (uint64_t)((ks * 4096) >> 4);   // two k-chunks per MMA
-            const uint32_t acc = ks > 0 ? 1u : 0u;
-            asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                         "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                         ::"r"(tmem), "l"(a), "l"(b), "r"(idesc), "r"(acc) : "memory");
-        }
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(&bar_mma)) : "memory");
     }
-    {
-        const uint32_t bar = smem_u32(&bar_mma);
+    {   // operands landed
+        const uint32_t bar = smem_u32(&bar_ld);
         asm volatile("{\n\t.reg .pred p;\n\tWAIT_%=:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t@p bra DONE_%=;\n\tbra WAIT_%=;\n\tDONE_%=:\n\t}"
                      ::"r"(bar), "r"(0u) : "memory");
     }
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int label = mt * 128 + warp * 32 + lane;
-    const float bias = bp[label];
-    const bool lab_ok = label < CZ_NLABEL;
-#pragma unroll 1
-    for (int q = 0; q < 4; q++) {
-        uint32_t v[32];
-        const uint32_t taddr = tmem + ((uint32_t)(warp * 32) << 16) + (uint32_t)(q * 32);
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                     "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                     "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                     : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                       "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-                       "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-                       "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-                     : "r"(taddr));
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+    float d[64];
 #pragma unroll
-        for (int j = 0; j < 32; j++) {
-            const int pos = nt * 128 + q * 32 + j;
-            if (lab_ok && pos < B) logits[(size_t)pos * CZ_NLABEL + label] = __uint_as_float(v[j]) + bias;
+    for (int i = 0; i < 64; i++) d[i] = 0.f;
+    const uint64_t da = gmma_desc(smem_u32(sA) + (uint32_t)(wg * 64 * 16), 2048), db = gmma_desc(smem_u32(sB), 2048);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 12; ks++)                                 // two k-chunks per MMA
+        Wgmma<128>::mma(d, da + (uint64_t)((ks * 4096) >> 4), db + (uint64_t)((ks * 4096) >> 4), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(d);
+    __syncthreads();                                                // both warpgroups are done reading the operands: they become sOut
+    {   // fragment -> sOut[position][label]: lane holds labels lr, lr + 8 and positions 8j + 2(lane%4) + {0, 1}
+        const int lr = wg * 64 + (warp & 3) * 16 + (lane >> 2), q = lane & 3;
+#pragma unroll
+        for (int j = 0; j < 16; j++) {
+            const int p = 8 * j + 2 * q;
+            sOut[p * FC_OUT_ROW + lr] = d[4 * j];
+            sOut[(p + 1) * FC_OUT_ROW + lr] = d[4 * j + 1];
+            sOut[p * FC_OUT_ROW + lr + 8] = d[4 * j + 2];
+            sOut[(p + 1) * FC_OUT_ROW + lr + 8] = d[4 * j + 3];
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(128u));
+    float bias[4];
+    bool lab_ok[4];
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+        const int label = mt * 128 + 32 * k + lane;
+        bias[k] = bp[label];
+        lab_ok[k] = label < CZ_NLABEL;
+    }
+#pragma unroll 1
+    for (int p = warp; p < 128; p += 8) {
+        const int pos = nt * 128 + p;
+        if (pos >= B) break;
+#pragma unroll
+        for (int k = 0; k < 4; k++)
+            if (lab_ok[k]) logits[(size_t)pos * CZ_NLABEL + mt * 128 + 32 * k + lane] = sOut[p * FC_OUT_ROW + 32 * k + lane] + bias[k];
+    }
 }
 
 constexpr int NPAD = 2112;   // 33 * 64 >= 2086
@@ -703,14 +643,14 @@ int cz_net_first_conv_mma(const uint8_t *canon_boards, int B, const void *w_frag
 
 int cz_net_first_conv_tc(const uint8_t *canon_boards, int B, const void *w_umma, const float *b1, void *out, void *stream) {
     if (!canon_boards || !w_umma || !b1 || !out || B <= 0) return CZ_EINVAL;
-    const int smem = 2 * TC_TILE_BYTES;   // 73 728 B > 48 KB default: opt in
+    const int smem = 2 * TC_TILE_BYTES + TC_OUT_BYTES;   // 106 496 B > 48 KB default: opt in
     if (cudaFuncSetAttribute(k_first_conv_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) return CZ_ECUDA;
     const long long tiles = ((long long)B * 90 + 127) / 128;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const long long grid = tiles < 3LL * sms ? tiles : 3LL * sms;    // persistent: three CTAs per SM (3 x 74 KB smem, 3 x 128 TMEM columns)
+    const long long grid = tiles < sms ? tiles : sms;                // persistent: one CTA per SM
     (void)b1;                                                         // the bias is row (centre tap, slot 15) of w_umma
-    k_first_conv_tc<<<(unsigned)grid, 128, smem, (cudaStream_t)stream>>>(canon_boards, B, reinterpret_cast<const uint4 *>(w_umma),
+    k_first_conv_tc<<<(unsigned)grid, 256, smem, (cudaStream_t)stream>>>(canon_boards, B, reinterpret_cast<const uint4 *>(w_umma),
                                                                         reinterpret_cast<__half *>(out));
     return cudaGetLastError() == cudaSuccess ? CZ_OK : CZ_ECUDA;
 }
@@ -756,8 +696,8 @@ int cz_net_heads(const void *x, int B, const float *wh, const float *bh, const f
 }
 
 
-// The heads for large batches: conv1x1 on mma.sync writing the policy features in the UMMA-tiled layout, value MLP on a side stream,
-// policy FC on tcgen05 (k_policy_fc_tc).  wp_tiled: dev fp16 [17 label tiles][24 k-chunks][128 labels][8] (labels >= 2086 zero),
+// The heads for large batches: conv1x1 on mma.sync writing the policy features in the wgmma-tiled layout, value MLP on a side stream,
+// policy FC on wgmma (k_policy_fc_tc).  wp_tiled: dev fp16 [17 label tiles][24 k-chunks][128 labels][8] (labels >= 2086 zero),
 // bp: dev f32 [2176]; hp_tiled scratch: fp16, ceil(B/128) * 49152 bytes, ZERO-INITIALISED by the caller (rows beyond B stay zero).
 int cz_net_heads_tc(const void *x, int B, const float *wh, const float *bh, const float *w1t, const float *b1, const float *w2, const float *b2,
                     const void *wp_tiled, const float *bp, void *hp_tiled_scratch, float *hv_scratch, float *logits, float *value, void *stream) {
@@ -782,7 +722,7 @@ int cz_net_heads_tc(const void *x, int B, const float *wh, const float *bh, cons
     if (cudaGetLastError() != cudaSuccess) return CZ_ECUDA;
     if (cudaEventRecord(ev_join[dev], side[dev]) != cudaSuccess) return CZ_ECUDA;
     dim3 grid((B + 127) / 128, 17);
-    k_policy_fc_tc<<<grid, 128, smem, st>>>((const uint4 *)hp_tiled_scratch, B, (const uint4 *)wp_tiled, bp, logits);
+    k_policy_fc_tc<<<grid, 256, smem, st>>>((const uint4 *)hp_tiled_scratch, B, (const uint4 *)wp_tiled, bp, logits);
     if (cudaGetLastError() != cudaSuccess) return CZ_ECUDA;
     if (cudaStreamWaitEvent(st, ev_join[dev], 0) != cudaSuccess) return CZ_ECUDA;
     return CZ_OK;
@@ -792,7 +732,7 @@ int cz_net_heads_tc(const void *x, int B, const float *wh, const float *bh, cons
 int cz_net_split_tf32(const float *y, float *hi, void *x2, long long n_pix, void *stream) {
     if (!y || !hi || !x2 || n_pix <= 0) return CZ_EINVAL;
     const long long n8 = n_pix * 16;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     long long blocks = (n8 + 255) / 256;
     if (blocks > 8LL * sms) blocks = 8LL * sms;          // grid-stride, 8 resident CTAs of 256 threads per SM
@@ -807,7 +747,7 @@ int cz_net_split_tf32(const float *y, float *hi, void *x2, long long n_pix, void
 int cz_net_epilogue_split(const float *t, const void *s, const float *bias, const float *skip, float *x, float *hi, void *x2, long long n_pix, void *stream) {
     if (!t || !bias || n_pix <= 0 || (!x && !hi) || ((hi == nullptr) != (x2 == nullptr))) return CZ_EINVAL;
     const long long n8 = n_pix * 16;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     long long blocks = (n8 + 255) / 256;
     if (blocks > 8LL * sms) blocks = 8LL * sms;

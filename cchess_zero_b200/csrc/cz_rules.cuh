@@ -1,4 +1,4 @@
-// cz_rules.cuh -- warp-cooperative xiangqi rules for sm_100a: bitboard move generation in the
+// cz_rules.cuh -- warp-cooperative xiangqi rules for sm_90a: bitboard move generation in the
 // reference's emission order, move application, flip and the 14-plane encode.
 //
 // One warp owns one position.  The piece identities sit in a 90-byte mailbox in shared memory (needed for the encode

@@ -1,6 +1,6 @@
 // cz_tower.cu -- the whole convolutional trunk of the policy-value network for a FEW positions (1..16) in ONE launch:
 // first conv3x3(14->128) + res_block_nums x [conv3x3 -> ReLU -> conv3x3 -> +skip -> ReLU] + the two 1x1 head convolutions
-// (policy_value_network.py:45-74, 151-162; batch norm folded into the weights), hand-written for sm_100a.
+// (policy_value_network.py:45-74, 151-162; batch norm folded into the weights), hand-written for sm_90a (H100).
 //
 // Why: play mode (BASELINE config 5) and any single-tree search evaluate one leaf (or a handful) per network call.  At batch 1
 // the library path is 15+ launches of ~5 us each, every one re-reading its weights; here the activations of a position never
@@ -8,21 +8,20 @@
 //
 // Shape: one thread-block CLUSTER of CL CTAs (CL = 1, 2, 4 or 8) per position; CTA r owns output channels
 // [r*128/CL, (r+1)*128/CL).  Per 3x3 convolution and CTA:
-//     D[128 rows][128/CL ch] (f32, TMEM) = sum over 9 taps of  A_tap[128][128] . B_tap[128][128/CL]      -- 72 tcgen05.mma (K = 16)
-//   * A = the position's activation image, fp16, resident in shared memory in the canonical K-major NO-SWIZZLE UMMA layout
+//     D[128 rows][128/CL ch] (f32, registers) = sum over 9 taps of  A_tap[128][128] . B_tap[128][128/CL]
+//   as two warpgroups, each 72 wgmma.mma_async m64nNk16 over its 64 rows (N = 128/CL).
+//   * A = the position's activation image, fp16, resident in shared memory in the canonical K-major NO-SWIZZLE layout
 //     [16 k-chunks of 8 channels][152 rows][8 halves]: with SBO = 128 B consecutive rows are 16 bytes apart in every chunk, so a
 //     3x3 tap is nothing but a START-ADDRESS OFFSET of (dr*11 + df) rows in the A descriptor -- no im2col, no copies.  Rows are
 //     image cells in a padded raster: cell (r, f) of the reference's [9][10] image sits in row 12 + r*11 + f; the 11th column and
 //     the rows above / below are zeros, which gives the convolution's zero padding for free (99 of the 128 MMA rows are cells).
 //   * B = this CTA's slice of the layer's weights, streamed tap by tap from L2 by TMA (cp.async.bulk.tensor, SASS UTMALDG)
 //     through a ring of shared-memory stages (full / empty mbarriers); the producer runs ahead across layers.
-//   * epilogue: 4 warps read their TMEM lanes (tcgen05.ld), add bias (+ the residual skip), ReLU, convert to fp16 and write the
-//     8-channel chunks of the NEXT layer's A image into the shared memory of ALL CL CTAs of the cluster (DSMEM stores), then
-//     signal every CTA's `act_ready` mbarrier; a CTA's MMA warp starts the next layer when all CL*4 epilogue warps have signalled.
-//     No cluster-wide barrier on the critical path.
-// Warp roles: 4*EW epilogue warps (warp w reads TMEM lane quarter w % 4 and column group w / 4 of this CTA's channels: the epilogue
-// is a dependent-issue chain per thread, so it is spread over up to 16 warps), then one TMA producer warp and one MMA issuer warp
-// (one elected lane each).
+//   * epilogue: each math thread adds bias (+ the residual skip) to its accumulator fragment, applies ReLU, converts to fp16 and
+//     writes its channel pairs of the NEXT layer's A image into the shared memory of ALL CL CTAs of the cluster (DSMEM stores);
+//     a CTA starts the next layer when all CL CTAs' slices have arrived on its `act_ready` mbarrier.  No cluster-wide barrier on
+//     the critical path.
+// Warp roles: 8 math warps (two warpgroups: MMA rows 0-63 and 64-127), then one TMA producer warp (one elected lane).
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -32,42 +31,36 @@
 #include <string.h>
 
 #include "../../include/cchess_b200.h"
+#include "cz_wgmma.cuh"
 
 namespace {
+
+using namespace cz_sm90;
 
 constexpr int ROWS = 152;                 // rows per k-chunk of an activation image (12 pad + 128 MMA rows + 12 pad)
 constexpr int P0 = 12;                    // row of image cell (0, 0)
 constexpr int LBO_A = ROWS * 16;          // bytes between k-chunks of A
 constexpr int A_BYTES = 16 * LBO_A;       // 38 912 B per activation image
+constexpr int NMATH = 256;                // two warpgroups
+constexpr int NMATH_WARPS = NMATH / 32;
+constexpr int NTHREADS = NMATH + 32;      // + the TMA producer warp
 
 // Byte offset of (8-channel chunk 0..15, raster row) inside an activation image: canonical K-major NO-SWIZZLE layout
-// [16 chunks][ROWS rows][16 B] (LBO = ROWS*16, SBO = 128).  A tap shift is a start-address offset of whole rows; a start that is not a
-// multiple of 8 rows makes every 128-byte core-matrix fetch straddle two shared-memory lines, which is what bounds the MMA phase
-// (64 cycles per M128 K16 MMA whatever N).  A K-major SWIZZLE_128B image (chunk c of row r at chunk position c ^ (r & 7), descriptor
-// base_offset 0: the hardware swizzles on absolute address bits) was implemented, verified against the same tests and measured SLOWER
-// (97 cycles per MMA: 32-byte K16 slices out of 128-byte rows) -- removed again.
+// [16 chunks][ROWS rows][16 B] (LBO = ROWS*16, SBO = 128).  A tap shift is a start-address offset of whole rows.
 __device__ __forceinline__ uint32_t img_off(int chunk, int row) { return (uint32_t)(chunk * LBO_A + row * 16); }
-__host__ __device__ constexpr int epi_groups(int CL) { return CL == 1 ? 4 : (CL == 2 ? 4 : 2); }      // default column groups of epilogue warps (EW)
-
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr, uint32_t lbo_bytes) {
-    // cute::UMMA::SmemDescriptor: start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | version=1 [46,48) | layout_type=0 (no swizzle) [61,64)
-    return (uint64_t)((smem_addr >> 4) & 0x3FFFu) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16) | ((uint64_t)(128u >> 4) << 32) | (1ull << 46);
-}
 
 __device__ __forceinline__ void mbar_init(uint64_t *b, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(b)), "r"(count));
 }
-// wait on a barrier whose arrivals all come from THIS CTA (threads, tcgen05.commit, TMA): CTA-scope acquire
+// wait on a barrier whose arrivals all come from THIS CTA (threads, TMA): CTA-scope acquire
 __device__ __forceinline__ void mbar_wait(uint64_t *b, uint32_t parity) {
     const uint32_t a = smem_u32(b);
     asm volatile("{\n\t.reg .pred p;\n\tWAIT_%=:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t@p bra DONE_%=;\n\tbra WAIT_%=;\n\tDONE_%=:\n\t}"
                  ::"r"(a), "r"(parity) : "memory");
 }
 // wait on a barrier that peer CTAs arrive on after writing OUR shared memory: cluster-scope acquire.  ptxas turns that into an
-// L1 invalidate (CCTL.IVALL) per successful wait -- measured as THE dominant stall when every waiter did it -- so exactly one
-// thread per CTA and layer waits this way; everybody else is ordered behind it with CTA-scope synchronisation.
+// L1 invalidate per successful wait, so exactly one thread per CTA and layer waits this way; everybody else is ordered behind it
+// with a CTA-scope named barrier.
 __device__ __forceinline__ void mbar_wait_cluster(uint64_t *b, uint32_t parity) {
     const uint32_t a = smem_u32(b);
     asm volatile("{\n\t.reg .pred p;\n\tWAIT_%=:\n\tmbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%0], %1;\n\t@p bra DONE_%=;\n\tbra WAIT_%=;\n\tDONE_%=:\n\t}"
@@ -75,6 +68,9 @@ __device__ __forceinline__ void mbar_wait_cluster(uint64_t *b, uint32_t parity) 
 }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t *b, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(b)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t *b) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(b)) : "memory");
 }
 // relaxed arrive on the barrier at the same shared-memory offset in CTA `rank`; the caller has issued fence.acq_rel.cluster
 __device__ __forceinline__ void mbar_arrive_remote(uint64_t *b, uint32_t rank) {
@@ -98,15 +94,25 @@ __device__ __forceinline__ void st_cluster_v4(uint32_t local_addr, uint32_t rank
     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(local_addr), "r"(rank));
     asm volatile("st.shared::cluster.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(ra), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
-// Async-proxy store of 16 bytes into CTA `rank`'s shared memory that completes 16 tx-bytes on THAT CTA's mbarrier: the designed
-// DSMEM producer -> consumer path.  Written through the async proxy, so the tensor cores (async proxy) need no proxy fence, and the
-// barrier completes by byte count: no arrive loop, no release fence on the critical path.
+__device__ __forceinline__ void st_cluster_b32(uint32_t local_addr, uint32_t rank, uint32_t v) {
+    uint32_t ra;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(local_addr), "r"(rank));
+    asm volatile("st.shared::cluster.b32 [%0], %1;" ::"r"(ra), "r"(v) : "memory");
+}
+// Async-proxy stores into CTA `rank`'s shared memory that complete their byte count on THAT CTA's mbarrier: the designed
+// DSMEM producer -> consumer path.  The barrier completes by byte count: no arrive loop, no release fence on the critical path.
 __device__ __forceinline__ void st_async_v4(uint32_t local_addr, uint32_t local_bar, uint32_t rank, uint4 v) {
     uint32_t ra, rb;
     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(local_addr), "r"(rank));
     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rb) : "r"(local_bar), "r"(rank));
-    asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v4.b32 [%0], {%1, %2, %3, %4}, [%5];"
+    asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.v4.b32 [%0], {%1, %2, %3, %4}, [%5];"
                  ::"r"(ra), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w), "r"(rb) : "memory");
+}
+__device__ __forceinline__ void st_async_b32(uint32_t local_addr, uint32_t local_bar, uint32_t rank, uint32_t v) {
+    uint32_t ra, rb;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(local_addr), "r"(rank));
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rb) : "r"(local_bar), "r"(rank));
+    asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];" ::"r"(ra), "r"(v), "r"(rb) : "memory");
 }
 __device__ __forceinline__ uint32_t cluster_rank() {
     uint32_t r;
@@ -116,6 +122,7 @@ __device__ __forceinline__ uint32_t cluster_rank() {
 __device__ __forceinline__ void cluster_sync_all() {
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
+__device__ __forceinline__ void math_sync() { asm volatile("bar.sync 1, %0;" ::"n"(NMATH) : "memory"); }   // the math warps only
 
 struct TowerArgs {
     const uint8_t *boards;     // [n][96] side-to-move canonical boards
@@ -131,22 +138,18 @@ struct TowerArgs {
 };
 
 // ASYNC_ST: image slices travel by st.async (complete_tx on the receiver's barrier) instead of generic stores + proxy fence + arrives.
-template <int CL, bool ASYNC_ST, int EW>
-__global__ void __launch_bounds__(64 + 128 * EW, 1) k_tower_small(const __grid_constant__ CUtensorMap wmap, TowerArgs a) {
+template <int CL, bool ASYNC_ST>
+__global__ void __launch_bounds__(NTHREADS, 1) k_tower_small(const __grid_constant__ CUtensorMap wmap, TowerArgs a) {
     constexpr uint32_t IMAGE_TX = 128u * 16u * 16u;        // bytes every CTA receives per image: 128 rows x 16 chunks x 16 B
-    constexpr int NC = 128 / CL;                           // output channels of this CTA
-    // EW = epilogue column groups: 4 * EW epilogue warps
-    constexpr int W = NC / EW;                             // channels per epilogue thread (8, 16 or 32)
-    constexpr int NEPI = 128 * EW, NTHREADS = NEPI + 64;
-    static_assert(W % 8 == 0 && W >= 8, "epilogue column groups");
+    constexpr int NC = 128 / CL;                           // output channels of this CTA (= wgmma N)
+    constexpr int W = NC / 2;                              // layer 0: channels per math thread (two column groups)
+    static_assert(W % 8 == 0 && W >= 8, "layer-0 column groups");
     constexpr int STAGE_BYTES = NC * 256;                  // one tap of this CTA's weight slice: [16 k-chunks][NC rows][8 halves]
     constexpr int S = CL == 1 ? 4 : (CL == 2 ? 8 : 16);    // ring depth
-    constexpr uint32_t TMEM_COLS = NC < 32 ? 32 : NC;
     extern __shared__ __align__(128) unsigned char smem[];
     unsigned char *bufX = smem, *bufY = smem + A_BYTES, *ring = smem + 2 * A_BYTES;
     float *s_bias = reinterpret_cast<float *>(ring + S * STAGE_BYTES);      // [n_layers][NC] this CTA's slice
-    __shared__ __align__(8) uint64_t full[S], empty[S], accum_full, act_ready[2];   // act_ready ping-pongs by layer parity: arrivals of consecutive layers never mix
-    __shared__ uint32_t tmem_slot;
+    __shared__ __align__(8) uint64_t full[S], empty[S], act_ready[2];       // act_ready ping-pongs by layer parity: arrivals of consecutive layers never mix
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const uint32_t rank = CL == 1 ? 0u : cluster_rank();
@@ -157,24 +160,16 @@ __global__ void __launch_bounds__(64 + 128 * EW, 1) k_tower_small(const __grid_c
     for (int i = tid; i < 2 * A_BYTES / 16; i += NTHREADS) reinterpret_cast<uint4 *>(smem)[i] = make_uint4(0, 0, 0, 0);   // zero images (padding rows stay zero)
     for (int i = tid; i < n_layers * NC; i += NTHREADS) s_bias[i] = a.bias[(i / NC) * 128 + rank * NC + (i % NC)];
     if (tid == 0) {
-        for (int s = 0; s < S; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        mbar_init(&accum_full, 1);
-        mbar_init(&act_ready[0], ASYNC_ST ? 1 : CL * 4 * EW);     // ASYNC_ST: one arrive.expect_tx by the MMA warp + IMAGE_TX bytes
-        mbar_init(&act_ready[1], ASYNC_ST ? 1 : CL * 4 * EW);
+        for (int s = 0; s < S; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], NMATH_WARPS); }
+        mbar_init(&act_ready[0], ASYNC_ST ? 1 : CL * NMATH_WARPS);      // ASYNC_ST: one arrive.expect_tx by thread 0 + IMAGE_TX bytes
+        mbar_init(&act_ready[1], ASYNC_ST ? 1 : CL * NMATH_WARPS);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)), "r"(TMEM_COLS));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-    }
     asm volatile("fence.proxy.async;" ::: "memory");     // the zeroed images (generic proxy) are what the tensor cores will read as padding
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
     if (CL > 1) cluster_sync_all();                      // every CTA's barriers and zeroed images exist before anyone writes remotely
-    const uint32_t tmem = tmem_slot;
 
-    if (warp == 4 * EW) {
+    if (warp == NMATH_WARPS) {
         // ===== TMA producer: taps of all layers, in order, as fast as the ring frees up =====
         if (lane == 0) {
             int stage = 0;
@@ -190,59 +185,13 @@ __global__ void __launch_bounds__(64 + 128 * EW, 1) k_tower_small(const __grid_c
                 }
             }
         }
-    } else if (warp == 4 * EW + 1) {
-        // ===== MMA issuer =====
-        if (lane == 0) {
-            // instruction descriptor: c_format F32 (1<<4), a/b F16 K-major, N>>3 at bit 17, M>>4 at bit 24
-            const uint32_t idesc = (1u << 4) | ((uint32_t)(NC >> 3) << 17) | (8u << 24);
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int L = 0; L < a.n_conv; L++) {
-                if (ASYNC_ST) mbar_expect_tx(&act_ready[L & 1], IMAGE_TX);      // our arrival + the byte count of image L
-                mbar_wait_cluster(&act_ready[L & 1], (uint32_t)((L >> 1) & 1));   // image L (this layer's input) is complete in OUR shared memory
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const bool tr = a.trace && blockIdx.x == 0;
-                if (tr) a.trace[L * 8 + 0] = clock64();
-                const uint32_t abase = smem_u32((L & 1) ? bufY : bufX);          // conv1 of a block reads X, conv2 reads Y
-                for (int t = 0; t < 9; t++) {
-                    mbar_wait(&full[stage], phase);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    if (tr && t == 0) a.trace[L * 8 + 1] = clock64();
-                    const int shift = (t / 3 - 1) * 11 + (t % 3 - 1);            // tap (dr, df) = a row offset in the padded raster
-                    const uint32_t arow = abase + (uint32_t)((P0 + shift) * 16);
-                    const uint32_t bbase = smem_u32(ring + stage * STAGE_BYTES);
-                    // Descriptors of the 8 K16 steps differ only in the 14-bit start-address field: one 32-bit add each from the tap's
-                    // base words (the issue loop is a dependent chain on the uniform datapath of ONE thread; building every descriptor
-                    // from scratch cost ~100 cycles per MMA, more than the MMA itself).
-                    const uint64_t da0 = umma_desc(arow, LBO_A);
-                    const uint64_t db0 = umma_desc(bbase, NC * 16);
-#pragma unroll
-                    for (int kk = 0; kk < 8; kk++) {                             // 128 input channels = 8 x K16
-                        const uint64_t da = da0 + (uint64_t)((kk * 2 * LBO_A) >> 4);
-                        const uint64_t db = db0 + (uint64_t)((kk * 2 * (NC * 16)) >> 4);
-                        if (t == 0 && kk == 0)
-                            asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 0, 0;\n\t"
-                                         "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                                         ::"r"(tmem), "l"(da), "l"(db), "r"(idesc) : "memory");
-                        else
-                            asm volatile("{\n\t.reg .pred p;\n\tsetp.eq.b32 p, 0, 0;\n\t"
-                                         "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-                                         ::"r"(tmem), "l"(da), "l"(db), "r"(idesc) : "memory");
-                    }
-                    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(&empty[stage])) : "memory");
-                    if (++stage == S) { stage = 0; phase ^= 1u; }
-                }
-                asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(&accum_full)) : "memory");
-                if (tr) a.trace[L * 8 + 2] = clock64();
-            }
-        }
     } else {
-        // ===== epilogue warps: thread = (column group cg, MMA row j = raster row P0 + j); warp % 4 = j / 32 = its TMEM lane quarter =====
-        const int j = tid & 127, cg = tid >> 7;              // row 0..127, column group 0..EW-1: channels [cg*W, (cg+1)*W) of this CTA's NC
-        const int rr = j / 11, ff = j - rr * 11;
-        const bool cell = rr < 9 && ff < 10;                 // a real image cell (else padding: must be written as zero)
-        // ---- layer 0: conv3x3(14 -> 128) straight from the board bytes (one-hot input: a gather-add of weight rows) ----
+        // ===== math warps: layer 0 by thread = (column group cg, MMA row j = raster row P0 + j) =====
         {
+            const int j = tid & 127, cg = tid >> 7;          // row 0..127, column group 0..1: channels [cg*W, (cg+1)*W) of this CTA's NC
+            const int rr = j / 11, ff = j - rr * 11;
+            const bool cell = rr < 9 && ff < 10;             // a real image cell (else padding: must be written as zero)
+            // conv3x3(14 -> 128) straight from the board bytes (one-hot input: a gather-add of weight rows)
             float acc[W];
 #pragma unroll
             for (int c = 0; c < W; c++) acc[c] = s_bias[cg * W + c];
@@ -287,67 +236,81 @@ __global__ void __launch_bounds__(64 + 128 * EW, 1) k_tower_small(const __grid_c
             }
             if (!ASYNC_ST) publish_image<CL>(&act_ready[0], lane);                // image 0
         }
-        // ---- residual tower epilogues ----
-        uint32_t fphase = 0;
+        // ===== residual tower: warpgroup wg multiplies MMA rows [64 wg, 64 wg + 64); this thread's accumulator rows are j0, j0 + 8 =====
+        const int wg = tid >> 7, q = lane & 3;
+        const int j0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+        bool cell[2];
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            const int j = j0 + 8 * h, rr = j / 11, ff = j - rr * 11;
+            cell[h] = rr < 9 && ff < 10;
+        }
+        float d[NC / 2];
+        int stage = 0;
+        uint32_t phase = 0;
         for (int L = 0; L < a.n_conv; L++) {
-            mbar_wait(&accum_full, fphase);
-            fphase ^= 1u;
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
             const bool tr = a.trace && blockIdx.x == 0 && tid == 0;
-            if (tr) a.trace[L * 8 + 3] = clock64();
+            if (tid == 0) {
+                if (ASYNC_ST) mbar_expect_tx(&act_ready[L & 1], IMAGE_TX);      // our arrival + the byte count of image L
+                mbar_wait_cluster(&act_ready[L & 1], (uint32_t)((L >> 1) & 1));   // image L (this layer's input) is complete in OUR shared memory
+            }
+            math_sync();
+            if (tr) a.trace[L * 8 + 0] = clock64();
+            const uint32_t abase = smem_u32((L & 1) ? bufY : bufX) + (uint32_t)((P0 + wg * 64) * 16);   // conv1 of a block reads X, conv2 reads Y
+            int prev = 0;
+            for (int t = 0; t < 9; t++) {
+                mbar_wait(&full[stage], phase);
+                if (tr && t == 0) a.trace[L * 8 + 1] = clock64();
+                const int shift = (t / 3 - 1) * 11 + (t % 3 - 1);                // tap (dr, df) = a row offset in the padded raster
+                // Descriptors of the 8 K16 steps differ only in the start-address field: one add each from the tap's base descriptor.
+                const uint64_t da0 = gmma_desc(abase + (uint32_t)(shift * 16), LBO_A);
+                const uint64_t db0 = gmma_desc(smem_u32(ring + stage * STAGE_BYTES), NC * 16);
+                wgmma_fence();
+#pragma unroll
+                for (int kk = 0; kk < 8; kk++)                                   // 128 input channels = 8 x K16
+                    Wgmma<NC>::mma(d, da0 + (uint64_t)((kk * 2 * LBO_A) >> 4), db0 + (uint64_t)((kk * 2 * (NC * 16)) >> 4), (t | kk) ? 1u : 0u);
+                wgmma_commit();
+                if (t > 0) {                                                     // the previous tap's MMAs are done: free its stage
+                    wgmma_wait<1>();
+                    if (lane == 0) mbar_arrive(&empty[prev]);
+                }
+                prev = stage;
+                if (++stage == S) { stage = 0; phase ^= 1u; }
+            }
+            wgmma_wait<0>();
+            fence_regs(d);
+            if (lane == 0) mbar_arrive(&empty[prev]);
+            if (tr) a.trace[L * 8 + 2] = a.trace[L * 8 + 3] = a.trace[L * 8 + 4] = clock64();
+            // ---- epilogue: bias (+ skip), ReLU, fp16, this thread's channel pairs of image L + 1 into every CTA of the cluster ----
             const bool second = L & 1;                        // conv2 of a block: + skip (the block input, still in X), result back into X
             unsigned char *dstbuf = second ? bufX : bufY;
-            // the skip operand (image L - 1, in X) arrived through the async proxy: observe its barrier before reading it generically
-            if (ASYNC_ST && second) mbar_wait(&act_ready[(L - 1) & 1], (uint32_t)(((L - 1) >> 1) & 1));
-            const float *bl = s_bias + (1 + L) * NC + cg * W;
-            uint32_t v[W];
-            const uint32_t taddr0 = tmem + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)(cg * W);
-            if (W == 8) {
-                asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                             : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]) : "r"(taddr0));
-            } else {
+            const float *bl = s_bias + (1 + L) * NC;
 #pragma unroll
-                for (int c16 = 0; c16 < W / 16; c16++) {
-                    uint32_t *u = v + c16 * 16;
-                    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-                                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                                 : "=r"(u[0]), "=r"(u[1]), "=r"(u[2]), "=r"(u[3]), "=r"(u[4]), "=r"(u[5]), "=r"(u[6]), "=r"(u[7]),
-                                   "=r"(u[8]), "=r"(u[9]), "=r"(u[10]), "=r"(u[11]), "=r"(u[12]), "=r"(u[13]), "=r"(u[14]), "=r"(u[15])
-                                 : "r"(taddr0 + (uint32_t)(c16 * 16)));
-                }
-            }
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            if (tr) a.trace[L * 8 + 4] = clock64();
+            for (int c8 = 0; c8 < NC / 8; c8++) {
+                const int chunk = (int)rank * (NC / 8) + c8;                     // 8-channel chunk of the full image
+                const float b0 = bl[c8 * 8 + 2 * q], b1 = bl[c8 * 8 + 2 * q + 1];
 #pragma unroll
-            for (int c8 = 0; c8 < W / 8; c8++) {
-                const int chunk = (int)rank * (NC / 8) + cg * (W / 8) + c8;          // 8-channel chunk of the full image
-                const uint32_t choff = img_off(chunk, P0 + j);
-                float f[8];
+                for (int h = 0; h < 2; h++) {
+                    const uint32_t off = img_off(chunk, P0 + j0 + 8 * h) + (uint32_t)(q * 4);
+                    float f0 = d[4 * c8 + 2 * h] + b0, f1 = d[4 * c8 + 2 * h + 1] + b1;
+                    if (second) {                                                // only this thread writes this word: it reads its own skip
+                        const float2 s = __half22float2(*reinterpret_cast<const __half2 *>(bufX + off));
+                        f0 += s.x; f1 += s.y;
+                    }
+                    const __half2 o = cell[h] ? __floats2half2_rn(fmaxf(f0, 0.f), fmaxf(f1, 0.f)) : __floats2half2_rn(0.f, 0.f);
+                    const uint32_t ov = *reinterpret_cast<const uint32_t *>(&o);
+                    if (ASYNC_ST) {
 #pragma unroll
-                for (int k = 0; k < 8; k++) f[k] = __uint_as_float(v[c8 * 8 + k]) + bl[c8 * 8 + k];
-                if (second) {
-                    const uint4 sk = *reinterpret_cast<const uint4 *>(bufX + choff);
-                    const __half2 *s2 = reinterpret_cast<const __half2 *>(&sk);
+                        for (int qi = 0; qi < CL; qi++)   // receivers in rotated order: at any moment the CL senders address CL different CTAs
+                            st_async_b32(smem_u32(dstbuf) + off, smem_u32(&act_ready[(L + 1) & 1]), (rank + 1u + (uint32_t)qi) & (uint32_t)(CL - 1), ov);
+                    } else if (CL == 1) *reinterpret_cast<uint32_t *>(dstbuf + off) = ov;
+                    else {
 #pragma unroll
-                    for (int k = 0; k < 4; k++) { const float2 s = __half22float2(s2[k]); f[2 * k] += s.x; f[2 * k + 1] += s.y; }
-                }
-                uint4 o;
-                __half2 *oh = reinterpret_cast<__half2 *>(&o);
-#pragma unroll
-                for (int k = 0; k < 4; k++)
-                    oh[k] = cell ? __floats2half2_rn(fmaxf(f[2 * k], 0.f), fmaxf(f[2 * k + 1], 0.f)) : __floats2half2_rn(0.f, 0.f);
-                if (ASYNC_ST) {
-#pragma unroll
-                    for (int qi = 0; qi < CL; qi++)     // receivers in rotated order: at any moment the CL senders address CL different CTAs
-                        st_async_v4(smem_u32(dstbuf) + choff, smem_u32(&act_ready[(L + 1) & 1]), (rank + 1u + (uint32_t)qi) & (uint32_t)(CL - 1), o);
-                } else if (CL == 1) *reinterpret_cast<uint4 *>(dstbuf + choff) = o;
-                else {
-#pragma unroll
-                    for (int q = 0; q < CL; q++) st_cluster_v4(smem_u32(dstbuf) + choff, (uint32_t)q, o);
+                        for (int r = 0; r < CL; r++) st_cluster_b32(smem_u32(dstbuf) + off, (uint32_t)r, ov);
+                    }
                 }
             }
             if (tr) a.trace[L * 8 + 5] = clock64();
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");       // our TMEM reads are done before the next layer's MMAs may overwrite
             if (!ASYNC_ST) publish_image<CL>(&act_ready[(L + 1) & 1], lane);       // image L + 1
         }
         // ---- heads: conv1x1 (128 -> 2 policy + 1 value) + bias + ReLU on the final image (in X), CTA 0 writes ----
@@ -356,8 +319,9 @@ __global__ void __launch_bounds__(64 + 128 * EW, 1) k_tower_small(const __grid_c
                 if (ASYNC_ST) mbar_expect_tx(&act_ready[a.n_conv & 1], IMAGE_TX);
                 mbar_wait_cluster(&act_ready[a.n_conv & 1], (uint32_t)((a.n_conv >> 1) & 1));                // the final image (index n_conv) is complete
             }
-            asm volatile("bar.sync 1, %0;" ::"n"(NEPI) : "memory");                // the epilogue warps, ordered behind thread 0's cluster-scope acquire
-            if (rank == 0 && cell && cg == 0) {
+            math_sync();                                                           // ordered behind thread 0's cluster-scope acquire
+            const int j = tid & 127, rr = j / 11, ff = j - rr * 11;
+            if (rank == 0 && tid < 128 && rr < 9 && ff < 10) {
                 float s0 = a.bh[0], s1 = a.bh[1], s2 = a.bh[2];
 #pragma unroll 4
                 for (int c8 = 0; c8 < 16; c8++) {
@@ -380,10 +344,8 @@ __global__ void __launch_bounds__(64 + 128 * EW, 1) k_tower_small(const __grid_c
         }
     }
     // ---- teardown: nobody leaves while a peer may still write into its shared memory ----
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
     if (CL > 1) cluster_sync_all();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(TMEM_COLS));
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *, const cuuint32_t *,
@@ -400,15 +362,15 @@ EncodeTiledFn encode_tiled() {
     return fn;
 }
 
-template <int CL, bool ASYNC_ST, int EW>
+template <int CL, bool ASYNC_ST>
 int launch_tower(const CUtensorMap &map, const TowerArgs &a, cudaStream_t st) {
     constexpr int NC = 128 / CL, S = CL == 1 ? 4 : (CL == 2 ? 8 : 16);
     const int n_layers = 1 + a.n_conv;
     const size_t smem = 2 * (size_t)A_BYTES + (size_t)S * NC * 256 + (size_t)n_layers * NC * 4;
-    if (cudaFuncSetAttribute(k_tower_small<CL, ASYNC_ST, EW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return CZ_ECUDA;
+    if (cudaFuncSetAttribute(k_tower_small<CL, ASYNC_ST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return CZ_ECUDA;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)(a.n_pos * CL));
-    cfg.blockDim = dim3(64 + 128 * EW);
+    cfg.blockDim = dim3(NTHREADS);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = st;
     cudaLaunchAttribute attr[1];
@@ -416,7 +378,7 @@ int launch_tower(const CUtensorMap &map, const TowerArgs &a, cudaStream_t st) {
     attr[0].val.clusterDim.x = CL; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, k_tower_small<CL, ASYNC_ST, EW>, map, a) == cudaSuccess ? CZ_OK : CZ_ECUDA;
+    return cudaLaunchKernelEx(&cfg, k_tower_small<CL, ASYNC_ST>, map, a) == cudaSuccess ? CZ_OK : CZ_ECUDA;
 }
 
 }  // namespace
@@ -460,7 +422,7 @@ int cz_net_tower_small(const uint8_t *canon_boards, int n_pos, int cluster, int 
             long long h[64 * 8];
             cudaStreamSynchronize(st);
             cudaMemcpy(h, dev, sizeof(h), cudaMemcpyDeviceToHost);
-            fprintf(stderr, "tower trace (clock64 deltas): layer: in_ready->w_ready, ->mma_issued, ->accum_seen(epi), ->tmem_loaded, ->stores_issued, ->next in_ready\n");
+            fprintf(stderr, "tower trace (clock64 deltas): layer: in_ready->w_ready, ->mma_issued, ->mma_done, ->(same), ->stores_issued, ->next in_ready\n");
             for (int L = 0; L < a.n_conv; L++) {
                 const long long *r = h + L * 8, nxt = L + 1 < a.n_conv ? h[(L + 1) * 8] : r[5];
                 fprintf(stderr, "  L%02d: %6lld %6lld %6lld %6lld %6lld %6lld | layer %6lld\n", L, r[1] - r[0], r[2] - r[1], r[3] - r[2], r[4] - r[3], r[5] - r[4], nxt - r[5], nxt - r[0]);
@@ -468,26 +430,12 @@ int cz_net_tower_small(const uint8_t *canon_boards, int n_pos, int cluster, int 
         }
     } dump{a, st, trace_dev, &trace_calls};
     static const bool generic_st = getenv("CCHESS_TOWER_ST") && !strcmp(getenv("CCHESS_TOWER_ST"), "generic");
-    if (generic_st) {
-        switch (cluster) {
-            case 1: return launch_tower<1, false, epi_groups(1)>(map, a, st);
-            case 2: return launch_tower<2, false, epi_groups(2)>(map, a, st);
-            case 4: return launch_tower<4, false, epi_groups(4)>(map, a, st);
-            default: return launch_tower<8, false, epi_groups(8)>(map, a, st);
-        }
-    }
-    // CCHESS_TOWER_EW = 1 | 2 | 4: epilogue column groups (4 * EW epilogue warps); default per cluster size (epi_groups)
-    static const int ew_env = getenv("CCHESS_TOWER_EW") ? atoi(getenv("CCHESS_TOWER_EW")) : 0;
-    const int ew = (ew_env == 1 || ew_env == 2 || (ew_env == 4 && cluster < 8)) ? ew_env : epi_groups(cluster);
-#define TOWER_CASE(CL_) \
-    case CL_: return ew == 1 ? launch_tower<CL_, true, 1>(map, a, st) : ew == 2 ? launch_tower<CL_, true, 2>(map, a, st) : launch_tower<CL_, true, (CL_ < 8 ? 4 : 2)>(map, a, st);
     switch (cluster) {
-        TOWER_CASE(1)
-        TOWER_CASE(2)
-        TOWER_CASE(4)
-        default: return ew == 1 ? launch_tower<8, true, 1>(map, a, st) : launch_tower<8, true, 2>(map, a, st);
+        case 1: return generic_st ? launch_tower<1, false>(map, a, st) : launch_tower<1, true>(map, a, st);
+        case 2: return generic_st ? launch_tower<2, false>(map, a, st) : launch_tower<2, true>(map, a, st);
+        case 4: return generic_st ? launch_tower<4, false>(map, a, st) : launch_tower<4, true>(map, a, st);
+        default: return generic_st ? launch_tower<8, false>(map, a, st) : launch_tower<8, true>(map, a, st);
     }
-#undef TOWER_CASE
 }
 
 }  // extern "C"

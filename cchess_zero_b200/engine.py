@@ -1,7 +1,7 @@
 """Python handle on the batched device engine (cz_engine_* in include/cchess_b200.h).
 
 torch is used for device buffers and streams only; all tree / rules work happens in the
-sm_100a kernels of csrc/cz_engine.cu."""
+sm_90a kernels of csrc/cz_engine.cu."""
 import ctypes as C
 
 import numpy as np

@@ -337,7 +337,7 @@ class SplitTf32Plan(InferencePlan):
 
 class NativePlan:
     """fp16 inference plan whose ends are the hand-written kernels of csrc/cz_net.cu:
-         board bytes --cz_net_first_conv--> [B,90,128] --library tcgen05 convs (residual tower)--> --cz_net_heads--> logits, value
+         board bytes --cz_net_first_conv--> [B,90,128] --library cuDNN convs (residual tower)--> --cz_net_heads--> logits, value
     Input is the engine's CZ_BOARD output (uint8 [B,96], the side-to-move-canonical board); the one-hot
     [9,10,14] tensor is never built.  Outputs are written straight into the float32 buffers the engine reads."""
 
@@ -345,9 +345,9 @@ class NativePlan:
     dtype = torch.uint8
 
     def __init__(self, net, max_batch, first_conv=None, owner=None):
-        """first_conv: "gather" (CUDA-core gather-add, k_first_conv; default: 12.8 us for 1024 positions in a graph), "tc" (tcgen05 + TMEM,
-        k_first_conv_tc: 12.1 us) or "mma" (mma.sync with the one-hot operand built in registers: 20.4 us -- every warp re-reads the
-        36 KB weight fragments from shared memory per 16-cell tile; kept as a tested alternative, measured and not adopted)."""
+        """first_conv: "gather" (CUDA-core gather-add, k_first_conv; the default), "tc" (wgmma,
+        k_first_conv_tc) or "mma" (mma.sync with the one-hot operand built in registers: every warp re-reads the 36 KB weight
+        fragments from shared memory per 16-cell tile).  "tc" and "mma" are tested alternatives to the default."""
         import ctypes as C
         from ._lib import lib
         self._C, self._lib = C, lib()
@@ -363,9 +363,9 @@ class NativePlan:
         self.x1 = torch.empty((max_batch, 9, 10, 128), dtype=torch.float16, device=dev)
         self.hp = torch.zeros((max_batch, 192), dtype=torch.float16, device=dev)
         self.hv = torch.zeros((max_batch, 96), dtype=torch.float32, device=dev)
-        # policy features in the UMMA-tiled layout of the tcgen05 policy FC (rows beyond the batch stay zero)
+        # policy features in the tiled operand layout of the wgmma policy FC (rows beyond the batch stay zero)
         self.hp_tiled = torch.zeros(((max_batch + 127) // 128, 24, 128, 8), dtype=torch.float16, device=dev)
-        self.heads = os.environ.get("CCHESS_HEADS", "tc")          # "tc": tcgen05 policy FC (batches >= 128); "mma": the mma.sync kernels
+        self.heads = os.environ.get("CCHESS_HEADS", "tc")          # "tc": wgmma policy FC (batches >= 128); "mma": the mma.sync kernels
 
     def _derive(self):
         """Kernel-layout copies of the ends' weights, derived from the folded base plan."""
@@ -375,7 +375,7 @@ class NativePlan:
             w, b = base.w_in                                                    # folded conv_in: [128,14,3,3] fp16
             w1 = w.float().permute(2, 3, 1, 0).reshape(9, 14, 128).to(torch.float16).contiguous()
             b1 = b.float().contiguous()
-            # tensor-core variant: K = tap*16 + piece code (codes 0 / 15 are zero rows), canonical K-major UMMA tile
+            # tensor-core variant: K = tap*16 + piece code (codes 0 / 15 are zero rows), canonical K-major no-swizzle tile
             # [k-chunk (18)][8-channel group (16)][channel in group (8)][k in chunk (8)]
             wpad = torch.zeros((9, 16, 128), dtype=torch.float16, device=dev)
             wpad[:, 1:15, :] = w1
@@ -385,7 +385,7 @@ class NativePlan:
             wp[:NLABEL, :180] = net.p_fc.weight.detach().to(torch.float16)
             bp = torch.zeros((2112,), dtype=torch.float32, device=dev)
             bp[:NLABEL] = net.p_fc.bias.detach().float()
-            # policy FC weights as tcgen05 operand tiles: [17 label tiles][24 k-chunks][128 labels][8 features]
+            # policy FC weights as wgmma operand tiles: [17 label tiles][24 k-chunks][128 labels][8 features]
             wp_pad = torch.zeros((2176, 192), dtype=torch.float16, device=dev)
             wp_pad[:2112] = wp
             bp_pad = torch.zeros((2176,), dtype=torch.float32, device=dev)
@@ -458,7 +458,7 @@ class NativePlan:
 class SmallTowerPlan:
     """fp16 plan for a FEW positions (play mode, single-tree search; BASELINE config 5): the whole convolutional trunk runs in
     ONE launch of csrc/cz_tower.cu (a thread-block cluster per position, activations resident in shared memory, weights streamed
-    by TMA, tcgen05.mma into TMEM), followed by the value MLP || policy FC kernels of csrc/cz_net.cu:
+    by TMA, wgmma accumulating in registers), followed by the value MLP || policy FC kernels of csrc/cz_net.cu:
         board bytes --cz_net_tower_small--> head features --cz_net_heads_fc--> logits, value            (3 kernels per evaluation)
     Same input / output contract as NativePlan (uint8 [B,96] canonical boards in, float32 logits / value written in place)."""
 
@@ -470,7 +470,7 @@ class SmallTowerPlan:
         import ctypes as C
         from ._lib import lib
         self._C, self._lib = C, lib()
-        self.cluster = int(cluster or os.environ.get("CCHESS_TOWER_CLUSTER", "4"))   # measured 70-72 us per evaluation for cluster sizes 2-8 at 1-16 positions (profiles/r02_tower_ncu_summary.md)
+        self.cluster = int(cluster or os.environ.get("CCHESS_TOWER_CLUSTER", "4"))
         assert self.cluster in (1, 2, 4, 8)
         self._base = InferencePlan(net, "fp16", owner=owner)
         self.fused = True

@@ -1,7 +1,7 @@
 """Host-side mirror of the reference's rules surface (module globals + GameBoard), backed by the
 CUDA library -- same names, argument meaning and error behaviour as main.py:23-91, 208-232, 579-1109.
 
-Every function that computes something (move lists, applied moves, encodes) launches the sm_100a
+Every function that computes something (move lists, applied moves, encodes) launches the sm_90a
 kernels through the C ABI (cz_*_batch); nothing here re-implements the rules on the CPU."""
 import ctypes as C
 

@@ -1,5 +1,5 @@
 /*
- * cchess_b200.h -- C ABI of the B200-native batched MCTS self-play engine.
+ * cchess_b200.h -- C ABI of the batched MCTS self-play engine (H100, sm_90a).
  *
  * The reference (chengstone/cchess-zero) is pure Python and has no FFI; this header is
  * the boundary a maintainer would bind from the reference's Python (ctypes stub in
@@ -198,8 +198,8 @@ int cz_engine_tree_signature(cz_engine *e, void *stream, int game, int64_t *out,
  *     w2 [256], b2 [1] (device pointers, so that weights can be refreshed under a captured CUDA graph): value MLP; wp fp16 [2112][192] / bp f32 [2112]: policy FC zero-padded; hp_scratch fp16 [B][192],
  *     hv_scratch f32 [B][96]. */
 int cz_net_first_conv(const uint8_t *canon_boards, int B, const void *w1, const float *b1, void *out, void *stream);
-/* Same result on the tcgen05 tensor cores: the one-hot im2col matrix is built in shared memory, the accumulators live in
- * TMEM.  w_umma: dev fp16, the weights in the canonical K-major UMMA layout [18 k-chunks][16 groups][8 channels][8 k]
+/* Same result on the Hopper tensor cores (wgmma): the one-hot im2col matrix is built in shared memory, the accumulators live in
+ * registers.  w_umma: dev fp16, the weights in the canonical K-major no-swizzle layout [18 k-chunks][16 groups][8 channels][8 k]
  * with k = tap*16 + piece code (code 0 rows are zero; row (centre tap, code 15) holds the bias, every other code-15 row is
  * zero); 36 864 bytes.  b1 is ignored (kept for signature symmetry with cz_net_first_conv). */
 int cz_net_first_conv_tc(const uint8_t *canon_boards, int B, const void *w_umma, const float *b1, void *out, void *stream);
@@ -223,7 +223,7 @@ int cz_host_choose_moves(int n_games, const uint8_t *live, const int32_t *n_chil
                          uint32_t *mt_states /* [B][626] */, int32_t *choice /* [B] */, double *probs /* [B][128] */, uint8_t *fallback /* [B] */,
                          int n_threads);
 
-/* cz_net_heads for large batches: policy FC on tcgen05 + TMEM (operands bulk-copied in the UMMA layout), 1x1 head convolution on
+/* cz_net_heads for large batches: policy FC on wgmma (operands bulk-copied in the K-major no-swizzle layout), 1x1 head convolution on
  * mma.sync, value MLP concurrently.  wp_tiled: dev fp16 [17 label tiles][24 k-chunks][128 labels][8 features] (labels >= 2086 zero),
  * bp f32 [2176]; hp_tiled_scratch: fp16, ceil(B/128) * 49152 bytes, zero-initialised once by the caller. */
 int cz_net_heads_tc(const void *x, int B, const float *wh, const float *bh, const float *w1t, const float *b1, const float *w2, const float *b2,
@@ -238,8 +238,8 @@ int cz_net_heads_fc(const void *hp, const float *hv, int B, const float *w1t, co
  * policy_value_network.py:45-74, 151-162 with batch norm folded: first conv3x3(14->128) from the canonical board bytes,
  * n_conv = 2*res_block_nums 3x3 convolutions (residual blocks), the two 1x1 head convolutions; output = the head features
  * hp fp16 [n_pos][192] / hv f32 [n_pos][96] that cz_net_heads_fc turns into logits and value.
- * One thread-block cluster of `cluster` (1, 2, 4, 8) CTAs per position: activations stay in shared memory (UMMA K-major layout,
- * 3x3 taps = descriptor start offsets), weights stream from L2 by TMA, tcgen05.mma accumulates in TMEM, epilogues exchange
+ * One thread-block cluster of `cluster` (1, 2, 4, 8) CTAs per position: activations stay in shared memory (K-major no-swizzle layout,
+ * 3x3 taps = descriptor start offsets), weights stream from L2 by TMA, wgmma accumulates in registers, epilogues exchange
  * channel slices through distributed shared memory.  See csrc/cz_tower.cu.
  *   w1     dev fp16 [9][14][128]   (as cz_net_first_conv);  bias dev f32 [1 + n_conv][128];  wh f32 [3][128], bh f32 [3]
  *   wblob  dev fp16, cz_net_tower_blob_bytes(n_conv) bytes, arranged for THIS cluster size:
