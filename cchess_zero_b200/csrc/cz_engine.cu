@@ -1155,15 +1155,36 @@ __device__ __forceinline__ void copy_block(uint32_t *__restrict__ dst, const uin
     }
 }
 
-__global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) k_play(Dev E) {
-    const int lane = threadIdx.x & 31, g = blockIdx.x * WARPS_PER_BLOCK + (threadIdx.x >> 5);
-    if (g >= E.B) return;
-    uint32_t *h = E.hdr + (size_t)g * HW;
-    uint8_t *b = E.root_board + (size_t)g * 96;
-    const int choice = E.st_choice[g];
-    if (choice < 0) { write_status(E, g, h, b, 0.0f, lane); return; }
-    const int rcnt = (int)h[H_ROOTCNT];
-    if (rcnt <= 0 || choice >= rcnt) { if (lane == 0) atomicOr(h + H_ERR, CZ_ERR_NOMOVES); write_status(E, g, h, b, 0.0f, lane); return; }
+// The game-state half of a move on the root (lane 0 only): board, side, restrict_round, ply, terminal flags (main.py:1522-1545)
+// and Zobrist key; the new root is N visits / ncnt children (-1: not expanded) at offset 0 of the other arena half, alloc words used.
+__device__ __forceinline__ void root_advance(const Dev &E, uint32_t *h, uint8_t *b, uint32_t flags, int cur, int src, int dst, int mover,
+                                             int cap, int rr_old, int ply_old, unsigned long long z_old, int N, int ncnt, uint32_t alloc) {
+    b[dst] = (uint8_t)mover;
+    b[src] = 0;
+    const int side = (flags & F_SIDE) ? 0 : 1;
+    const int rr = cap == 0 ? rr_old + 1 : 0;
+    uint32_t f = (flags & ~(F_ACTIVE | 6u | F_SIDE | F_CUR)) | (side ? F_SIDE : 0u) | (cur ? 0u : F_CUR);
+    // main.py:1532-1545: king missing -> winner, else restrict_round >= 60 -> tie
+    if (cap == 1) f = (f & ~0xF00u) | (1u << 8) | (2u << 10);          // 'K' captured: black wins
+    else if (cap == 8) f = (f & ~0xF00u) | (1u << 8) | (1u << 10);     // 'k' captured: red wins
+    else if (rr >= 60) f = (f & ~0xF00u) | (2u << 8);
+    const unsigned long long z = z_old ^ E.zob[mover * 96 + src] ^ E.zob[mover * 96 + dst] ^ E.zob[95] ^ (cap ? E.zob[cap * 96 + dst] : 0ull);
+    h[H_FLAGS] = f;
+    h[H_RR] = (uint32_t)rr;
+    h[H_PLY] = (uint32_t)(ply_old + 1);
+    h[H_ROOTN] = (uint32_t)N;
+    h[H_ROOTCNT] = (uint32_t)ncnt;
+    h[H_ROOTBASE] = 0;
+    h[H_ALLOC] = alloc;
+    h[H_DONE] = 0;
+    h[H_TARGET] = 0;
+    h[H_PLEN] = 0;
+    h[H_HASHLO] = (uint32_t)z; h[H_HASHHI] = (uint32_t)(z >> 32);
+    if (alloc > h[H_MAXALLOC]) h[H_MAXALLOC] = alloc;
+}
+
+// Play child `choice` (0 <= choice < rcnt) of game g's expanded root; the whole warp takes part.
+__device__ __forceinline__ void play_child(const Dev &E, int g, uint32_t *h, uint8_t *b, int choice, int rcnt, int lane) {
     const uint32_t flags = h[H_FLAGS];
     const int cur = (flags & F_CUR) ? 1 : 0;
     const uint32_t *old = arena_half(E, g, cur);
@@ -1216,32 +1237,68 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) k_play(Dev E) {
         }
     }
     __syncwarp();
-    if (lane == 0) {
-        b[dst] = (uint8_t)mover;
-        b[src] = 0;
-        const int side = (flags & F_SIDE) ? 0 : 1;
-        const int rr = cap == 0 ? rr_old + 1 : 0;
-        uint32_t f = (flags & ~(F_ACTIVE | 6u | F_SIDE | F_CUR)) | (side ? F_SIDE : 0u) | (cur ? 0u : F_CUR);
-        // main.py:1532-1545: king missing -> winner, else restrict_round >= 60 -> tie
-        if (cap == 1) f = (f & ~0xF00u) | (1u << 8) | (2u << 10);          // 'K' captured: black wins
-        else if (cap == 8) f = (f & ~0xF00u) | (1u << 8) | (1u << 10);     // 'k' captured: red wins
-        else if (rr >= 60) f = (f & ~0xF00u) | (2u << 8);
-        const unsigned long long z = z_old ^ E.zob[mover * 96 + src] ^ E.zob[mover * 96 + dst] ^ E.zob[95] ^ (cap ? E.zob[cap * 96 + dst] : 0ull);
-        h[H_FLAGS] = f;
-        h[H_RR] = (uint32_t)rr;
-        h[H_PLY] = (uint32_t)(ply_old + 1);
-        h[H_ROOTN] = (uint32_t)N;
-        h[H_ROOTCNT] = (uint32_t)ncnt;
-        h[H_ROOTBASE] = 0;
-        h[H_ALLOC] = alloc;
-        h[H_DONE] = 0;
-        h[H_TARGET] = 0;
-        h[H_PLEN] = 0;
-        h[H_HASHLO] = (uint32_t)z; h[H_HASHHI] = (uint32_t)(z >> 32);
-        if (alloc > h[H_MAXALLOC]) h[H_MAXALLOC] = alloc;
-    }
+    if (lane == 0) root_advance(E, h, b, flags, cur, src, dst, mover, cap, rr_old, ply_old, z_old, N, ncnt, alloc);
     __syncwarp();
     write_status(E, g, h, b, q, lane);
+}
+
+__global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) k_play(Dev E) {
+    const int lane = threadIdx.x & 31, g = blockIdx.x * WARPS_PER_BLOCK + (threadIdx.x >> 5);
+    if (g >= E.B) return;
+    uint32_t *h = E.hdr + (size_t)g * HW;
+    uint8_t *b = E.root_board + (size_t)g * 96;
+    const int choice = E.st_choice[g];
+    if (choice < 0) { write_status(E, g, h, b, 0.0f, lane); return; }
+    const int rcnt = (int)h[H_ROOTCNT];
+    if (rcnt <= 0 || choice >= rcnt) { if (lane == 0) atomicOr(h + H_ERR, CZ_ERR_NOMOVES); write_status(E, g, h, b, 0.0f, lane); return; }
+    play_child(E, g, h, b, choice, rcnt, lane);
+}
+
+// ---- play a given move (any move legal at the root, searched or not): MCTS_tree.update_tree(act) for a move the tree did not
+// choose (human_move, main.py:1412-1418).  moves[g] = src | dst << 7, 0xFFFF = leave game g alone.  An expanded root plays the child
+// that carries the move exactly as k_play does; an unexpanded root (fresh reset, or re-rooted onto an unvisited child) checks the
+// move against the position's legal moves and moves on to an empty tree at the new position (no search is run for it, unlike
+// human_move).  A move that is not legal there, or any move in a finished game, sets CZ_ERR_ILLEGAL and leaves the game as it was.
+__global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) k_play_moves(Dev E, const uint16_t *moves) {
+    __shared__ WarpSmem smem[WARPS_PER_BLOCK];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, g = blockIdx.x * WARPS_PER_BLOCK + w;
+    if (g >= E.B) return;
+    uint32_t *h = E.hdr + (size_t)g * HW;
+    uint8_t *b = E.root_board + (size_t)g * 96;
+    const uint32_t mv = moves[g];
+    if (mv == 0xFFFFu) { write_status(E, g, h, b, 0.0f, lane); return; }
+    const uint32_t flags = h[H_FLAGS];
+    const int rcnt = (int)h[H_ROOTCNT];
+    if (F_TERM(flags) == 0) {
+        if (rcnt > 0) {
+            const uint32_t rcs = (uint32_t)((rcnt + 7) & ~7);
+            const uint32_t *meta = arena_half(E, g, (flags & F_CUR) ? 1 : 0) + h[H_ROOTBASE] + HDR + 3 * rcs;
+            for (int i0 = 0; i0 < rcnt; i0 += 32) {
+                const unsigned m = __ballot_sync(CZ_FULL, i0 + lane < rcnt && (meta[i0 + lane] & 0xFFFFu) == mv);
+                if (m) { play_child(E, g, h, b, i0 + __ffs(m) - 1, rcnt, lane); return; }
+            }
+        } else {
+            WarpSmem &S = smem[w];
+            for (int i = lane; i < 90; i += 32) S.board[i] = b[i];
+            __syncwarp();
+            int n = cz::warp_legal_moves(S.board, (flags & F_SIDE) ? 1 : 0, S.moves, S.scratch, lane);
+            if (n > 136) n = 136;
+            bool hit = false;
+            for (int i = lane; i < n; i += 32) hit |= S.moves[i] == mv;
+            if (__any_sync(CZ_FULL, hit)) {
+                const int src = mv & 127, dst = (mv >> 7) & 127;
+                if (lane == 0) {
+                    const unsigned long long z = (unsigned long long)h[H_HASHLO] | ((unsigned long long)h[H_HASHHI] << 32);
+                    root_advance(E, h, b, flags, (flags & F_CUR) ? 1 : 0, src, dst, b[src], b[dst], (int)h[H_RR], (int)h[H_PLY], z, 0, -1, 0u);
+                }
+                __syncwarp();
+                write_status(E, g, h, b, 0.0f, lane);
+                return;
+            }
+        }
+    }
+    if (lane == 0) atomicOr(h + H_ERR, CZ_ERR_ILLEGAL);
+    write_status(E, g, h, b, 0.0f, lane);
 }
 
 // ---- stateless batched rules ------------------------------------------------------------
@@ -1796,6 +1853,23 @@ int cz_engine_play_status(cz_engine *e, void *stream, const int32_t *child_index
 }
 
 int cz_engine_play(cz_engine *e, void *stream, const int32_t *child_index) { return cz_engine_play_status(e, stream, child_index, nullptr); }
+
+int cz_engine_play_moves(cz_engine *e, void *stream, const uint16_t *moves, uint8_t *status) {
+    if (!e || !moves) return fail(CZ_EINVAL, "cz_engine_play_moves: null");
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t B = (size_t)e->d.B;
+    CUDA_TRY(cudaSetDevice(e->device));
+    uint16_t *hm = reinterpret_cast<uint16_t *>(e->h_choice);          // pinned staging of cz_engine_play (B * 4 bytes)
+    uint16_t *dm = reinterpret_cast<uint16_t *>(e->d.st_choice);
+    memcpy(hm, moves, B * 2);
+    CUDA_TRY(cudaMemcpyAsync(dm, hm, B * 2, cudaMemcpyHostToDevice, st));
+    k_play_moves<<<nblk(e->d.B, WARPS_PER_BLOCK), 32 * WARPS_PER_BLOCK, 0, st>>>(e->d, dm);
+    CUDA_TRY(cudaGetLastError());
+    if (status) CUDA_TRY(cudaMemcpyAsync(e->h_status, e->d.st_status, B * CZ_STATUS_BYTES, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));   // h_choice is reused by the next call
+    if (status) memcpy(status, e->h_status, B * CZ_STATUS_BYTES);
+    return CZ_OK;
+}
 
 int cz_engine_status_packed(cz_engine *e, void *stream, uint8_t *status) {
     if (!e || !status) return fail(CZ_EINVAL, "cz_engine_status_packed: null");

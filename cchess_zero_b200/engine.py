@@ -155,6 +155,17 @@ class Engine:
         check(lib().cz_engine_play_status(self.h, _stream(), _hp(ci), _hp(rec)), "cz_engine_play_status")
         return self._unpack_status(rec) if want_status else None
 
+    def play_moves(self, moves, want_status=True):
+        """Play the given move (src | dst << 7; 0xFFFF = none) in every game, searched at the root or not: the opponent's move in a
+        game where each player keeps its own tree (update_tree for a move the tree did not choose).  A move that is not legal at the
+        root, or any move in a finished game, sets the ILLEGAL error flag and leaves that game unchanged (cz_engine_play_moves)."""
+        mv = np.ascontiguousarray(moves, dtype=np.uint16)
+        assert mv.shape == (self.B,)
+        self.launches += 1
+        rec = np.zeros((self.B, STATUS_BYTES), dtype=np.uint8) if want_status else None
+        check(lib().cz_engine_play_moves(self.h, _stream(), _hp(mv), _hp(rec)), "cz_engine_play_moves")
+        return self._unpack_status(rec) if want_status else None
+
     @staticmethod
     def _unpack_status(rec):
         tail = np.ascontiguousarray(rec[:, 96:112]).view(np.int32)

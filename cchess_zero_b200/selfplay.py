@@ -51,6 +51,46 @@ def _label_table():
     return _LABEL_OF
 
 
+def sample_moves(n_children, visits, live, temperature, mt_states, exploration, n_threads=1):
+    """get_action's move choice (main.py:1339-1348) for a batch of games, bit-identical to the numpy calls: pi = softmax(1/T *
+    log(visits)) in float64, then RandomState.choice(p = pi) -- with exploration, p = 0.75 * pi + 0.25 * RandomState.dirichlet(0.3).
+    n_children [B] int32 / visits [B,128]: the root statistics; live [B]: the games that choose (others get -1); temperature: a
+    scalar or one value per game; mt_states [B,626]: one legacy MT19937 state per game, advanced in place.  Returns choice [B] int32."""
+    B = len(n_children)
+    choice = np.full(B, -1, dtype=np.int32)
+    inv_t = (1.0 / temperature) if np.ndim(temperature) == 0 else (1.0 / np.asarray(temperature, dtype=np.float64))[:, None]
+    with np.errstate(divide="ignore", invalid="ignore"):
+        # softmax(1/T * log(visits)) of main.py:1341, 1111-1116.  log / exp / max are element-wise or exact, so they are
+        # taken over the whole [B,128] batch at once (padding: visits 0 -> -inf -> exp 0); the order-sensitive row sum, the
+        # Dirichlet / choice draws and the cumulative sums happen per game in csrc/cz_host.cu, operation for operation what
+        # numpy does for `probs /= np.sum(probs)`, RandomState.dirichlet and RandomState.choice (main.py:1345-1348).
+        lv = inv_t * np.log(visits.astype(np.int64))
+        valid = np.arange(MAXCHILD)[None, :] < n_children[:, None]
+        lv[~valid] = -np.inf
+        ex = np.ascontiguousarray(np.exp(lv - np.max(lv, axis=1, keepdims=True)))
+    probs = np.empty((B, MAXCHILD), dtype=np.float64)
+    fallback = np.zeros(B, dtype=np.uint8)
+    live8 = np.ascontiguousarray(live, dtype=np.uint8)
+    nn = np.ascontiguousarray(n_children, dtype=np.int32)
+    from ._lib import lib
+    import ctypes as C
+    vp = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
+    rcode = lib().cz_host_choose_moves(B, vp(live8), vp(nn), vp(ex), 1 if exploration else 0, vp(mt_states), vp(choice), vp(probs),
+                                       vp(fallback), n_threads)
+    if rcode:
+        raise EngineError("cz_host_choose_moves failed (%d)" % rcode)
+    for g in np.nonzero(fallback)[0]:
+        # a probability vector numpy would reject (NaN priors ...): let numpy raise exactly what the reference would raise
+        n = int(nn[g])
+        rs = np.random.RandomState()
+        rs.set_state(("MT19937", mt_states[g, :624].copy(), int(mt_states[g, 624]), 0, 0.0))
+        pr = ex[g, :n] / np.sum(ex[g, :n])
+        choice[g] = int(rs.choice(n, p=pr))          # (the Dirichlet draws were consumed by the native sampler, as in the reference)
+        st_ = rs.get_state()
+        mt_states[g, :624], mt_states[g, 624] = st_[1], st_[2]
+    return choice
+
+
 class GameRecord:
     """(s, pi, z) tuples of one finished game in the reference's format (selfplay, main.py:1493-1554).
 
@@ -354,12 +394,12 @@ class SelfPlay:
             cs.wait_stream(side)
         self.graph = g
 
-    def _search_pipeline(self):
+    def _search_pipeline(self, m):
         e = self.engine
         A, Bn = self.lanes
-        for p in np.unique(self.playouts[self.live]):
-            e.begin_search(int(p), (self.live & (self.playouts == p)).astype(np.uint8))
-        pmax = int(self.playouts[self.live].max()) if self.live.any() else 0
+        for p in np.unique(self.playouts[m]):
+            e.begin_search(int(p), (m & (self.playouts == p)).astype(np.uint8))
+        pmax = int(self.playouts[m].max()) if m.any() else 0
         A.engine.wave(A.nn_in, A.logits, A.value)      # prologue: lane A's first leaves
         waves = 1
         while True:
@@ -415,13 +455,13 @@ class SelfPlay:
             self._bucket_graphs[n] = g
         g.replay()
 
-    def _search_compact(self):
+    def _search_compact(self, m):
         e = self.engine
         if self.plan is not None and hasattr(self.plan, "refresh_if_stale"):
             self.plan.refresh_if_stale()
-        for p in np.unique(self.playouts[self.live]):
-            e.begin_search(int(p), (self.live & (self.playouts == p)).astype(np.uint8))
-        pmax = int(self.playouts[self.live].max()) if self.live.any() else 0
+        for p in np.unique(self.playouts[m]):
+            e.begin_search(int(p), (m & (self.playouts == p)).astype(np.uint8))
+        pmax = int(self.playouts[m].max()) if m.any() else 0
         waves = 0
         while True:
             e.wave_compact(self.nn_stage, self.nn_in, self.logits, self.value)
@@ -458,18 +498,20 @@ class SelfPlay:
             self._eval(self.nn_in)
         self.graph = g
 
-    def search(self):
-        """MCTS_tree.main for every live game: `playouts[g]` playouts each."""
+    def search(self, mask=None):
+        """MCTS_tree.main for every live game (or every game with mask[g], e.g. the games where one player of a match is to move):
+        `playouts[g]` playouts each."""
+        m = self.live if mask is None else np.asarray(mask, dtype=bool)
         if self.lanes is not None:
-            return self._search_pipeline()
+            return self._search_pipeline(m)
         if self.compact:
-            return self._search_compact()
+            return self._search_compact(m)
         e = self.engine
         if self.plan is not None and hasattr(self.plan, "refresh_if_stale"):
             self.plan.refresh_if_stale()       # weights trained / restored since the last search (the graph reads them in place)
-        for p in np.unique(self.playouts[self.live]):
-            e.begin_search(int(p), (self.live & (self.playouts == p)).astype(np.uint8))
-        pmax = int(self.playouts[self.live].max()) if self.live.any() else 0
+        for p in np.unique(self.playouts[m]):
+            e.begin_search(int(p), (m & (self.playouts == p)).astype(np.uint8))
+        pmax = int(self.playouts[m].max()) if m.any() else 0
         waves = 0
         while True:
             if self.graph is not None:
@@ -493,40 +535,12 @@ class SelfPlay:
         e = self.engine
         self.search()
         rc = e.root_children(want_wpq=False)                      # n, moves, visits: what get_action reads (main.py:1339)
-        choice = np.full(self.B, -1, dtype=np.int32)
         live = np.nonzero(self.live)[0]
         if (rc["n"][live] <= 0).any():
             e.raise_on_error()
             raise EngineError("game %d has no root children" % int(live[np.argmax(rc["n"][live] <= 0)]))
-        with np.errstate(divide="ignore", invalid="ignore"):
-            # softmax(1/T * log(visits)) of main.py:1341, 1111-1116.  log / exp / max are element-wise or exact, so they are
-            # taken over the whole [B,128] batch at once (padding: visits 0 -> -inf -> exp 0); the order-sensitive row sum, the
-            # Dirichlet / choice draws and the cumulative sums happen per game in csrc/cz_host.cu, operation for operation what
-            # numpy does for `probs /= np.sum(probs)`, RandomState.dirichlet and RandomState.choice (main.py:1345-1348).
-            lv = (1.0 / self.temperature) * np.log(rc["visits"].astype(np.int64))
-            valid = np.arange(MAXCHILD)[None, :] < rc["n"][:, None]
-            lv[~valid] = -np.inf
-            ex = np.ascontiguousarray(np.exp(lv - np.max(lv, axis=1, keepdims=True)))
-        probs = np.empty((self.B, MAXCHILD), dtype=np.float64)
-        fallback = np.zeros(self.B, dtype=np.uint8)
-        live8 = np.ascontiguousarray(self.live, dtype=np.uint8)
         nn = np.ascontiguousarray(rc["n"], dtype=np.int32)
-        from ._lib import lib
-        import ctypes as C
-        vp = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
-        rcode = lib().cz_host_choose_moves(self.B, vp(live8), vp(nn), vp(ex), 1 if self.exploration else 0, vp(self._mt), vp(choice), vp(probs),
-                                           vp(fallback), self._threads)
-        if rcode:
-            raise EngineError("cz_host_choose_moves failed (%d)" % rcode)
-        for g in np.nonzero(fallback)[0]:
-            # a probability vector numpy would reject (NaN priors ...): let numpy raise exactly what the reference would raise
-            n = int(rc["n"][g])
-            rs = np.random.RandomState()
-            rs.set_state(("MT19937", self._mt[g, :624].copy(), int(self._mt[g, 624]), 0, 0.0))
-            pr = ex[g, :n] / np.sum(ex[g, :n])
-            choice[g] = int(rs.choice(n, p=pr))          # (the Dirichlet draws were consumed by the native sampler, as in the reference)
-            st_ = rs.get_state()
-            self._mt[g, :624], self._mt[g, 624] = st_[1], st_[2]
+        choice = sample_moves(nn, rc["visits"], self.live, self.temperature, self._mt, self.exploration, self._threads)
         if self.keep_records:
             entry = dict(boards=self.boards, n=nn, moves=rc["moves"], visits=rc["visits"], choice=choice)
             for g in live:
@@ -859,6 +873,19 @@ class cchess_main(object):
                 self.mcts.reload()
         print("Using time {} s".format(time.time() - start_time))
         return zip(states, mcts_probs, z), len(z)
+
+    # ---- evaluation (main.py:1207-1222, commented out in the reference; not called from run()) ---------------------------
+    def policy_evaluate(self, n_games=10, opponent=None):
+        """Plays n_games (even: colour-swapped pairs) of this network against `opponent` (another policy_value_network; None = a
+        search-only opponent with zero logits and zero value -- the reference's stub used pure MCTS with random rollouts, which
+        this engine does not have), self.playout_counts playouts per move and self.search_threads, all games at once
+        (arena.Match).  Prints the stub's line and returns win_ratio = (win + 0.5 tie) / n_games."""
+        from .arena import Match, UniformEvaluator
+        r = Match(self.policy_value_netowrk, UniformEvaluator() if opponent is None else opponent, n_games, self.playout_counts,
+                  search_threads=self.search_threads).run()
+        win_ratio = 1.0 * (r.wins + 0.5 * r.draws) / n_games
+        print("num_playouts:{}, win: {}, lose: {}, tie:{}".format(self.playout_counts, r.wins, r.losses, r.draws))
+        return win_ratio
 
     # ---- batched bridge: many games at once on this rank's GPU ---------------------------------------
     def selfplay_many(self, n_games, seeds=None, arena_words=0):

@@ -50,6 +50,7 @@ extern "C" {
 #define CZ_ERR_DEPTH 4       /* search path deeper than the path stack */
 #define CZ_ERR_ARENA 8       /* tree arena exhausted */
 #define CZ_ERR_CHILDREN 16   /* more than CZ_MAXCHILD moves */
+#define CZ_ERR_ILLEGAL 32    /* cz_engine_play_moves: move not legal at the game's root (game left unchanged) */
 
 const char *cz_last_error(void);
 int cz_version(void);
@@ -172,6 +173,15 @@ int cz_engine_play(cz_engine *e, void *stream, const int32_t *child_index /* [B]
  * 104 Q (f32) of the move just played = MCTS_tree.Q(act), main.py:1350 | 108 N of the new root i32. */
 #define CZ_STATUS_BYTES 112
 int cz_engine_play_status(cz_engine *e, void *stream, const int32_t *child_index /* [B] */, uint8_t *status /* host [B][112] or NULL */);
+/* Play a given MOVE in every game (MCTS_tree.update_tree(act) for a move the tree did not choose, human_move main.py:1412-1418 --
+ * e.g. the opponent's move in a match where each player keeps its own tree).  moves[g] = src | dst << 7 as cz_engine_root_children
+ * returns it, 0xFFFF = leave game g alone.  Expanded root: exactly cz_engine_play of the child that carries the move.  Unexpanded
+ * root (fresh reset, or re-rooted onto an unvisited child): the move is checked against the legal moves of the side to move and
+ * the game advances to an empty tree at the new position (q = 0; unlike human_move, no search is run first).  A move that is not
+ * legal at the root, or any move in a finished game, sets CZ_ERR_ILLEGAL in that game's error word and leaves the game unchanged;
+ * the other games are played.  Status records as cz_engine_play_status (q = MCTS_tree.Q(act) of the child played). */
+int cz_engine_play_moves(cz_engine *e, void *stream, const uint16_t *moves /* [B] host, 0xFFFF = no move */,
+                         uint8_t *status /* host [B][CZ_STATUS_BYTES] or NULL */);
 int cz_engine_status_packed(cz_engine *e, void *stream, uint8_t *status /* host [B][112] */);
 
 /* Game status (cchess_main.check_end main.py:1380-1392): HOST buffers, any may be NULL; synchronises.
