@@ -23,7 +23,7 @@ import torch
 
 from . import rules
 from ._lib import MT_WORDS, NLABEL, EngineError
-from .selfplay import SelfPlay, sample_moves
+from .selfplay import SelfPlay, network_selfplay, sample_moves
 
 NO_MOVE = 0xFFFF
 
@@ -129,9 +129,7 @@ class _Player:
         self.colour, self.lo, self.hi = colour, lo, lo + n
         kw = dict(auto_reset=False, keep_records=False, search_threads=search_threads, arena_words=arena_words)
         if hasattr(evaluator, "native_plan"):                       # a policy_value_network: its own plan and precision
-            fp16 = evaluator.precision == "fp16"
-            self.sp = SelfPlay(n, None, playouts, plan_factory=(lambda r: evaluator.native_plan(r)) if fp16 else (lambda r: evaluator.plan()),
-                               **kw)
+            self.sp = network_selfplay(evaluator, n, playouts, **kw)
         else:                                                       # a device callable (nn_in) -> (logits, value)
             self.sp = SelfPlay(n, evaluator, playouts, **kw)
         self.sp.capture_graph()

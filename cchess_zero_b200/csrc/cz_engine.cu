@@ -76,6 +76,8 @@ struct Labels {
     char text[CZ_NLABEL][4];
     int16_t of[CZ_NSQ * CZ_NSQ];
     int32_t unflipped[CZ_NLABEL];
+    int16_t mirror[CZ_NLABEL];     // label of the left-right mirrored move (file x -> 8 - x); replay-batch augmentation
+    bool mirror_ok;                // the table is closed under the mirror and an involution
     Labels() {
         int n = 0;
         auto put = [&](int l1, int n1, int l2, int n2) {
@@ -107,6 +109,14 @@ struct Labels {
             int s = (9 - (text[i][1] - '0')) * 9 + (text[i][0] - 'a'), d = (9 - (text[i][3] - '0')) * 9 + (text[i][2] - 'a');
             unflipped[i] = of[s * CZ_NSQ + d];
         }
+        mirror_ok = true;
+        for (int i = 0; i < CZ_NLABEL; i++) {
+            int s = (text[i][1] - '0') * 9 + (8 - (text[i][0] - 'a')), d = (text[i][3] - '0') * 9 + (8 - (text[i][2] - 'a'));
+            mirror[i] = of[s * CZ_NSQ + d];
+            if (mirror[i] < 0) mirror_ok = false;
+        }
+        for (int i = 0; i < CZ_NLABEL && mirror_ok; i++)
+            if (mirror[mirror[i]] != i) mirror_ok = false;
     }
 };
 const Labels &labels() { static Labels L; return L; }
@@ -1326,6 +1336,45 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) k_encode(const uint8_t *
     cz::warp_encode<T>(S.board, sides[g], out + (size_t)g * CZ_ENC_LEN, lane);
 }
 
+// ---- replay mini-batch assembly (cz_replay_batch) ---------------------------------------------
+__device__ int16_t d_mirror_label[CZ_NLABEL];
+
+// One warp per output row r: the ring record rows[r] (canonical board, n sparse (label, prob) pairs, z) becomes the
+// training tuple policy_update reads (main.py:1164-1166): planes = state_to_positions of the board (warp_encode with side 0:
+// the board is already canonical), pi = the dense [2086] vector, z.  mirror[r] != 0: the board is mirrored left to right
+// (file x -> 8 - x) before it is encoded and every probability goes to the mirrored move's label.  Row indices and record
+// contents are validated by the caller; out-of-range values are skipped, never trapped on.
+__global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) k_replay_batch(const uint8_t *boards, const uint8_t *n, const int16_t *idx,
+                                                                      const float *prob, const float *z, int cap, const int32_t *rows,
+                                                                      const uint8_t *mirror, int m, float *planes, float *pi, float *zout) {
+    __shared__ uint8_t sboard[WARPS_PER_BLOCK][96];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, r = blockIdx.x * WARPS_PER_BLOCK + w;
+    if (r >= m) return;
+    const int row = rows[r];
+    if (row < 0 || row >= cap) return;
+    const bool mir = mirror != nullptr && mirror[r] != 0;
+    const uint8_t *b = boards + (size_t)row * CZ_NSQ;
+    uint8_t *s = sboard[w];
+    for (int i = lane; i < CZ_NSQ; i += 32) {
+        const int y = i / 9, x = i - y * 9;
+        s[i] = b[mir ? y * 9 + 8 - x : i];
+    }
+    __syncwarp();
+    cz::warp_encode<float>(s, 0, planes + (size_t)r * CZ_ENC_LEN, lane);
+    // a pi row is 8344 bytes: 8-byte aligned for every r, so the zero fill is 1043 float2 stores
+    float *pr = pi + (size_t)r * CZ_NLABEL;
+    for (int i = lane; i < CZ_NLABEL / 2; i += 32) reinterpret_cast<float2 *>(pr)[i] = make_float2(0.0f, 0.0f);
+    __syncwarp();                                      // the zeros land before any lane scatters over them
+    const int cnt = min((int)n[row], CZ_MAXCHILD);
+    for (int k = lane; k < cnt; k += 32) {
+        int l = idx[(size_t)row * CZ_MAXCHILD + k];
+        if (l < 0 || l >= CZ_NLABEL) continue;
+        if (mir) l = d_mirror_label[l];
+        pr[l] = prob[(size_t)row * CZ_MAXCHILD + k];
+    }
+    if (lane == 0) zout[r] = z[row];
+}
+
 __global__ void k_apply(uint8_t *boards, const uint16_t *moves, int n, uint8_t *captured) {
     const int g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= n) return;
@@ -1541,6 +1590,37 @@ int cz_encode_batch(int device, const uint8_t *boards, const uint8_t *sides, int
     rc = cz_encode_dev(db, ds, n, dout, CZ_F32, nullptr);
     if (rc) return rc;
     CUDA_TRY(cudaMemcpy(out, dout, (size_t)n * CZ_ENC_LEN * 4, cudaMemcpyDeviceToHost));
+    return CZ_OK;
+}
+
+int cz_mirror_labels(int16_t *out) {
+    if (!out) return fail(CZ_EINVAL, "cz_mirror_labels: null");
+    if (!labels().mirror_ok) return fail(CZ_EINVAL, "cz_mirror_labels: the label table is not closed under the left-right mirror");
+    memcpy(out, labels().mirror, sizeof(labels().mirror));
+    return CZ_OK;
+}
+
+int cz_replay_batch(const uint8_t *boards, const uint8_t *n, const int16_t *idx, const float *prob, const float *z, int cap,
+                    const int32_t *rows, const uint8_t *mirror, int m, float *planes, float *pi, float *zout, void *stream) {
+    if (m < 0 || cap < 0) return fail(CZ_EINVAL, "cz_replay_batch: negative size");
+    if (mirror) {                                     // the mirror label table, uploaded once per device (synchronous)
+        static bool uploaded[64] = {false};
+        int dev = 0;
+        CUDA_TRY(cudaGetDevice(&dev));
+        if (dev < 0 || dev >= 64) return fail(CZ_EINVAL, "cz_replay_batch: device index");
+        if (!uploaded[dev]) {
+            if (!labels().mirror_ok) return fail(CZ_EINVAL, "cz_replay_batch: the label table is not closed under the left-right mirror");
+            CUDA_TRY(cudaMemcpyToSymbol(d_mirror_label, labels().mirror, sizeof(labels().mirror)));
+            uploaded[dev] = true;
+        }
+    }
+    if (m == 0) return CZ_OK;
+    if (!boards || !n || !idx || !prob || !z || !rows || !planes || !pi || !zout) return fail(CZ_EINVAL, "cz_replay_batch: null");
+    if (cap == 0) return fail(CZ_EINVAL, "cz_replay_batch: empty ring");
+    if (((uintptr_t)planes & 15) || ((uintptr_t)pi & 7)) return fail(CZ_EINVAL, "cz_replay_batch: planes must be 16-byte and pi 8-byte aligned");
+    k_replay_batch<<<nblk(m, WARPS_PER_BLOCK), 32 * WARPS_PER_BLOCK, 0, (cudaStream_t)stream>>>(boards, n, idx, prob, z, cap, rows, mirror, m,
+                                                                                               planes, pi, zout);
+    CUDA_TRY(cudaGetLastError());
     return CZ_OK;
 }
 

@@ -652,6 +652,10 @@ class policy_value_network(object):
         x = torch.as_tensor(np.asarray(positions, dtype=np.float32)).reshape(-1, 9, 10, 14).to(self.device)
         pi = torch.as_tensor(np.asarray(probs, dtype=np.float32)).to(self.device)
         z = torch.as_tensor(np.asarray(winners, dtype=np.float32)).reshape(-1, 1).to(self.device)
+        return self.train_step_device(x, pi, z, learning_rate)
+
+    def train_step_device(self, x, pi, z, learning_rate):
+        """train_step on a mini-batch that is already on the device: x f32 [B,9,10,14], pi f32 [B,2086], z f32 [B,1]."""
         accuracy, loss = train_step_module(self.net, self.opt, x, pi, z, learning_rate, self.c_l2, self.global_norm)
         self.net.eval()
         self.weights_version += 1

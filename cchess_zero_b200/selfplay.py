@@ -602,6 +602,15 @@ class SelfPlay:
         return sorted(self.finished, key=lambda t: t[0])
 
 
+def network_selfplay(network, n_games, playouts, **kw):
+    """SelfPlay evaluated by a policy_value_network: an fp16 network runs its native plan (board bytes in, the hand-written first
+    convolution and heads), any other precision its own inference plan.  Either plan follows the network's weights_version, so a
+    search after train_step / restore sees the new weights."""
+    if network.precision == "fp16":
+        return SelfPlay(n_games, None, playouts, plan_factory=lambda r: network.native_plan(r), **kw)
+    return SelfPlay(n_games, None, playouts, plan_factory=lambda r: network.plan(), **kw)
+
+
 # =================================================================================================
 # Reference-shaped facade: cchess_main (main.py:1118-1554).  One game at a time through MCTS_tree,
 # exactly the call sequence of the reference, so main.py's train loop runs unchanged on top of it.
@@ -668,6 +677,7 @@ class cchess_main(object):
 
     # ---- training (main.py:1157-1205) ------------------------------------------------------------
     def policy_update(self):
+        from .train import explained_variance, next_lr_multiplier, policy_kl
         mini_batch = random.sample(self.data_buffer, self.batch_size)
         state_batch = [d[0] for d in mini_batch]
         mcts_probs_batch = [d[1] for d in mini_batch]
@@ -679,22 +689,14 @@ class cchess_main(object):
             accuracy, loss, self.global_step = self.policy_value_netowrk.train_step(
                 state_batch, mcts_probs_batch, winner_batch, self.learning_rate * self.lr_multiplier)
             new_probs, new_v = self.mcts.forward(state_batch)
-            with np.errstate(all="ignore"):
-                kl_tmp = old_probs * (np.log((old_probs + 1e-10) / (new_probs + 1e-10)))
-            # main.py:1178-1182 drops the terms whose str() is 'nan' or 'inf' -- and therefore KEEPS '-inf' (logits are used as
-            # probabilities, so negative old_probs are routine and a row sum can legitimately be -inf)
-            kl = np.mean([np.sum(line[~(np.isnan(line) | np.isposinf(line))]) for line in kl_tmp])
+            kl = policy_kl(old_probs, new_probs)
             if kl > self.kl_targ * 4:
                 break
         self.policy_value_netowrk.save(self.global_step)
         print("train using time {} s".format(time.time() - start_time))
-        if kl > self.kl_targ * 2 and self.lr_multiplier > 0.1:
-            self.lr_multiplier /= 1.5
-        elif kl < self.kl_targ / 2 and self.lr_multiplier < 10:
-            self.lr_multiplier *= 1.5
-        wb = np.array(winner_batch)
-        explained_var_old = 1 - np.var(wb - old_v.flatten()) / np.var(wb)
-        explained_var_new = 1 - np.var(wb - new_v.flatten()) / np.var(wb)
+        self.lr_multiplier = next_lr_multiplier(kl, self.kl_targ, self.lr_multiplier)
+        explained_var_old = explained_variance(winner_batch, old_v)
+        explained_var_new = explained_variance(winner_batch, new_v)
         msg = "kl:{:.5f},lr_multiplier:{:.3f},loss:{},accuracy:{},explained_var_old:{:.3f},explained_var_new:{:.3f}".format(
             kl, self.lr_multiplier, loss, accuracy, explained_var_old, explained_var_new)
         print(msg)

@@ -78,6 +78,24 @@ int cz_encode_batch(int device, const uint8_t *boards, const uint8_t *sides, int
 int cz_legal_moves_dev(const uint8_t *boards, const uint8_t *sides, int n, uint16_t *moves, int32_t *counts, void *stream);
 int cz_encode_dev(const uint8_t *boards, const uint8_t *sides, int n, void *out, int dtype, void *stream);
 
+/* ---- replay buffer -> training mini-batch (cchess_main.policy_update's data path, main.py:1160-1166 + run() 1236-1239) ----
+ * The ring holds cap records in device arrays: boards u8 [cap][90] (side-to-move canonical), n u8 [cap], idx i16 [cap][128]
+ * (label indices), prob f32 [cap][128] (visit probabilities), z f32 [cap].  Output row r is ring record rows[r]:
+ *   planes f32 [m][9][10][14]  = MCTS_tree.state_to_positions(state) (main.py:547-557, incl. its rank*9+file indexing)
+ *   pi     f32 [m][2086]       = the dense pi vector: zeros, prob[k] at label idx[k] for k < n
+ *   zout   f32 [m]             = z
+ * mirror (dev u8 [m] or NULL): rows with mirror[r] != 0 are mirrored left to right (file x -> 8 - x) -- the board before it
+ * is encoded, each probability to the mirrored move's label (cz_mirror_labels).  rows, mirror and all arrays are DEVICE
+ * pointers; planes 16-byte, pi 8-byte aligned.  Asynchronous on `stream`, no allocation: capturable in a CUDA graph -- except
+ * the first call with a mirror array on a device, which uploads the 4 KB mirror table (synchronous; m may be 0 for that).
+ * Row indices and record contents (n <= 128, 0 <= idx < 2086) are the caller's to validate; invalid ones are skipped.
+ * CZ_EINVAL: m < 0, cap < 0, a NULL array with m > 0, cap == 0 with m > 0, misaligned outputs. */
+int cz_replay_batch(const uint8_t *boards, const uint8_t *n, const int16_t *idx, const float *prob, const float *z, int cap,
+                    const int32_t *rows, const uint8_t *mirror, int m, float *planes, float *pi, float *zout, void *stream);
+/* The left-right mirror of every label: out[i] = label of label i with both files x -> 8 - x (host [2086]).  The table is
+ * closed under the mirror and an involution (checked when the label table is built; CZ_EINVAL otherwise). */
+int cz_mirror_labels(int16_t *out /* [2086] host */);
+
 /* ---- the batched engine: n_games independent (GameBoard, MCTS_tree) pairs resident in HBM ---- */
 typedef struct cz_engine cz_engine;
 
