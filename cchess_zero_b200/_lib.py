@@ -61,17 +61,14 @@ def _sig(L):
     L.cz_engine_counters.argtypes = [vp, vp, vp]
     L.cz_engine_tree_signature.argtypes = [vp, vp, i32, vp, i64, vp]
     L.cz_net_first_conv.argtypes = [vp, i32, vp, vp, vp, vp]
-    L.cz_net_first_conv_tc.argtypes = [vp, i32, vp, vp, vp, vp]
-    L.cz_net_first_conv_mma.argtypes = [vp, i32, vp, vp, vp]
     L.cz_net_heads.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.cz_host_choose_moves.argtypes = [i32, vp, vp, vp, i32, vp, vp, vp, vp, i32]
     L.cz_net_heads_tc.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.cz_net_heads_fc.argtypes = [vp, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
-    L.cz_net_split_tf32.argtypes = [vp, vp, vp, i64, vp]
     L.cz_net_epilogue_split.argtypes = [vp, vp, vp, vp, vp, vp, vp, i64, vp]
     L.cz_net_tower_blob_bytes.argtypes = [i32]
     L.cz_net_tower_blob_bytes.restype = i64
-    L.cz_net_tower_small.argtypes = [vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.cz_net_tower_small.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp]
 
 
 def lib():

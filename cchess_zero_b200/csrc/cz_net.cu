@@ -7,19 +7,19 @@
 //                       gather-add of weight rows: out[cell][:] = b + sum over the 3x3 neighbourhood of W[tap][piece][:].
 //                       The [9][10][14] tensor (and the reference's rank*9+file indexing, main.py:550-555) is never
 //                       materialised: image cell (r, f) reads canonical board byte r*9+f.
-//   k_first_conv_tc   : the same layer on wgmma (one-hot im2col operand built in shared memory).
 //   k_head_conv_mma   : conv1x1(128->3)+bias+ReLU (policy 2 ch + value 1 ch) as one streaming pass on mma.sync (hi+lo fp16
 //                       weight split: fp32-weight accuracy); writes the policy features hp either row-major fp16 [B][192]
-//                       (flatten order (h, w, c), zero padded) or directly as wgmma operand tiles.  k_head_conv: round-1 SIMT form.
+//                       (flatten order (h, w, c), zero padded) or directly as wgmma operand tiles.
 //   k_value_mlp       : 90 -> 256 ReLU -> 1 tanh, 8 positions per CTA, all 90 weights of a hidden unit requested up front.
 //   k_policy_fc_tc    : logits[B][2086] = hp . Wp^T + bp on wgmma; both operands arrive as 48 KB bulk async copies
 //                       (cp.async.bulk) already in the operand layout; fp32 logits stored 128 B per warp and position.
-//   k_policy_fc       : the same on mma.sync m16n8k16 (small batches, row-major hp).
+//                       Batches of 128 rows or more (cz_net_heads_tc).
+//   k_policy_fc       : the same on mma.sync m16n8k16 (smaller batches and the small-batch trunk, row-major hp).
+//   k_epilogue_split  : the f32 epilogue of one convolution of the fp32-accurate plan (net.py: SplitTf32Plan) fused with the
+//                       tf32 hi / lo operand split for the next one.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdlib.h>
-#include <string.h>
 
 #include "../../include/cchess_b200.h"
 #include "cz_wgmma.cuh"
@@ -77,225 +77,6 @@ __device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], 
                  : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
 }
 
-// ------------------------------------------------------------------------------------------
-// first convolution on mma.sync with the ONE-HOT operand built in registers (alternative; measured 20.4 us vs 12.8 us for the gather-add
-// at 1024 positions: each warp streams the whole 36 KB of weight fragments from shared memory per 16-cell tile -- not adopted).
-//   D[16 cells][128 ch] = A[16][144] . B[144][128],  K = 9 taps x 16 piece slots (slot 0 = empty -> zero weight row; slot 15 of the
-//   centre tap is a constant 1 against the bias row, as in the wgmma variant).  A never exists anywhere: lane (g, t) of the warp
-//   derives its m16n8k16 fragment words for tap `tap` from the two piece codes of its rows g and g + 8 -- a 1.0 in the half that
-//   matches the code, zero otherwise (~10 ALU instructions per tap).  B is the weight matrix pre-arranged on the host in FRAGMENT
-//   order [k-step 9][n-tile 16][lane 32][2 words], copied once per CTA into shared memory: one conflict-free LDS.64 per MMA.
-//   A CTA (8 warps) handles 4 positions = 24 row tiles, 3 per warp.
-// ------------------------------------------------------------------------------------------
-constexpr int FCM_POS = 4;
-__global__ void __launch_bounds__(256) k_first_conv_mma(const uint8_t *__restrict__ boards, int B, const uint2 *__restrict__ wfrag /* [9][16][32] */,
-                                                         __half *__restrict__ out /* [B][90][128] */) {
-    __shared__ uint2 sW[9 * 16 * 32];                          // 36 864 B
-    __shared__ uint8_t pb[FCM_POS][11 * 12 + 12];              // zero-bordered images: pb[(r+1)*12 + f+1] = canonical board byte r*9+f (r < 9, f < 10)
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, t = lane & 3;
-    const int pos0 = blockIdx.x * FCM_POS;
-    for (int i = tid; i < 9 * 16 * 32 / 2; i += 256) reinterpret_cast<uint4 *>(sW)[i] = __ldg(reinterpret_cast<const uint4 *>(wfrag) + i);
-    for (int i = tid; i < FCM_POS * 144; i += 256) {
-        const int p = i / 144, j = i - p * 144;
-        uint8_t v = 0;
-        if (j < 132 && pos0 + p < B) {
-            const int r = j / 12 - 1, f = j % 12 - 1;
-            if (r >= 0 && r < 9 && f >= 0 && f < 10) v = boards[(size_t)(pos0 + p) * 96 + r * 9 + f];   // the reference's cell <- s[rank*9+file]
-        }
-        pb[p][j] = v;
-    }
-    __syncthreads();
-#pragma unroll 1
-    for (int tile = warp; tile < FCM_POS * 6; tile += 8) {
-        const int p = tile / 6, mt = tile - p * 6;
-        if (pos0 + p >= B) break;
-        const int c0 = mt * 16 + g, c1 = c0 + 8;               // this lane's two rows (cells); rows >= 90 are padding
-        const int r0 = c0 / 10, f0 = c0 - r0 * 10, r1 = c1 / 10, f1 = c1 - r1 * 10;
-        const uint8_t *q0 = pb[p] + r0 * 12 + f0, *q1 = pb[p] + r1 * 12 + f1;   // top-left of the 3x3 windows
-        float acc[16][4];
-#pragma unroll
-        for (int nt = 0; nt < 16; nt++) { acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f; }
-#pragma unroll
-        for (int tap = 0; tap < 9; tap++) {
-            const int off = (tap / 3) * 12 + (tap % 3);
-            const int pc0 = c0 < 90 ? q0[off] : 0, pc1 = c1 < 90 ? q1[off] : 0;
-            uint32_t a[4];
-            const uint32_t one0 = 0x3C00u << ((pc0 & 1) * 16), one1 = 0x3C00u << ((pc1 & 1) * 16);
-            a[0] = (pc0 >> 1) == t ? one0 : 0u;                // k = 2t, 2t+1   <-> codes 0..7
-            a[1] = (pc1 >> 1) == t ? one1 : 0u;
-            a[2] = (pc0 >> 1) == t + 4 ? one0 : 0u;            // k = 2t+8, 2t+9 <-> codes 8..15
-            a[3] = (pc1 >> 1) == t + 4 ? one1 : 0u;
-            if (tap == 4 && t == 3) { if (c0 < 90) a[2] |= 0x3C000000u; if (c1 < 90) a[3] |= 0x3C000000u; }   // slot 15 of the centre tap: 1 x bias row
-            const uint2 *wk = sW + tap * 16 * 32 + lane;
-#pragma unroll
-            for (int nt = 0; nt < 16; nt++) {
-                const uint2 bw = wk[nt * 32];
-                const uint32_t b[2] = {bw.x, bw.y};
-                mma16816(acc[nt], a, b);
-            }
-        }
-        __half *o0 = out + ((size_t)(pos0 + p) * 90 + c0) * 128 + t * 2, *o1 = out + ((size_t)(pos0 + p) * 90 + c1) * 128 + t * 2;
-#pragma unroll
-        for (int nt = 0; nt < 16; nt++) {
-            if (c0 < 90) *reinterpret_cast<__half2 *>(o0 + nt * 8) = __floats2half2_rn(fmaxf(acc[nt][0], 0.f), fmaxf(acc[nt][1], 0.f));
-            if (c1 < 90) *reinterpret_cast<__half2 *>(o1 + nt * 8) = __floats2half2_rn(fmaxf(acc[nt][2], 0.f), fmaxf(acc[nt][3], 0.f));
-        }
-    }
-}
-
-// ------------------------------------------------------------------------------------------
-// first convolution on the Hopper tensor cores (wgmma), one 128-cell tile per CTA iteration.
-//   D[128 cells][128 ch] (f32, registers) = A[128][144] . B[144][128],  K = 9 taps x 16 "piece slots"
-//   A is ONE-HOT and never exists in global memory: row r (its cell's 3x3 neighbourhood, one 16-wide slot per tap with a 1.0 at the
-//   piece code; code 0 = empty / off-board hits an all-zero weight row) is built straight into shared memory in the canonical
-//   K-major no-swizzle layout by two threads (taps 0-4 and 5-8); B (the folded conv weights, same layout, prepared once on the host)
-//   is copied from L2.  Two warpgroups, one per 64-row half, each issue 9 wgmma m64n128k16 (f16 in, f32 accumulate); the epilogue
-//   applies ReLU and converts to fp16 straight from the accumulator registers.
-// Shared-memory operand layout (both A and B): [k-chunk of 8 halves (18)][8-row group (16)][row in group (8)][8 halves]
-//   -> core matrix = 128 contiguous bytes, SBO (next 8-row group) = 128 B, LBO (next k-chunk) = 2048 B.
-// ------------------------------------------------------------------------------------------
-constexpr int TC_TILE_BYTES = 18 * 16 * 128;   // 36 864 B per operand
-constexpr int TC_OUT_BYTES = 128 * 256;        // fp16 output tile, staged for coalesced stores
-
-// Persistent: each CTA copies B once, then walks tiles blockIdx.x, +gridDim.x, ... (one CTA per SM: 162 registers x 256 threads).
-// The bias rides in the GEMM: slot 15 of the centre tap is a constant 1 in A and the bias row
-// in B, so the epilogue is ReLU + fp16 convert only.
-__global__ void __launch_bounds__(256) k_first_conv_tc(const uint8_t *__restrict__ boards, int B, const uint4 *__restrict__ wB /* TC_TILE_BYTES */,
-                                                           __half *__restrict__ out /* [B][90][128] */) {
-    extern __shared__ __align__(128) unsigned char smem_tc[];
-    unsigned char *sA = smem_tc, *sB = smem_tc + TC_TILE_BYTES, *sOut = smem_tc + 2 * TC_TILE_BYTES;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
-    const long long total = (long long)B * 90;
-    const long long tiles = (total + 127) / 128;
-
-    for (int i = tid; i < TC_TILE_BYTES / 16; i += 256) reinterpret_cast<uint4 *>(sB)[i] = __ldg(wB + i);   // B operand, once
-    const uint64_t da = gmma_desc(smem_u32(sA) + (uint32_t)(wg * 64 * 16), 2048), db = gmma_desc(smem_u32(sB), 2048);
-    const int row = tid & 127, t_lo = wg ? 5 : 0, t_hi = wg ? 9 : 5;   // this thread builds taps [t_lo, t_hi) of A row `row`
-    unsigned char *rowp = sA + row * 16;
-
-    // piece codes of the 3x3 neighbourhood of cell c (0 = empty / outside the board / beyond the batch)
-    auto load_codes = [&](long long c, int (&pc)[9]) {
-#pragma unroll
-        for (int t = 0; t < 9; t++) pc[t] = 0;
-        if (c < total) {
-            const int pos = (int)(c / 90), cell = (int)(c - (long long)pos * 90);
-            const int r = cell / 10, f = cell - r * 10;
-            const uint8_t *bd = boards + (size_t)pos * 96;
-#pragma unroll
-            for (int t = 0; t < 9; t++) {
-                const int rr = r + t / 3 - 1, ff = f + t % 3 - 1;
-                if (rr >= 0 && rr < 9 && ff >= 0 && ff < 10) pc[t] = __ldg(bd + rr * 9 + ff);   // the reference's cell <- s[rank*9+file]
-            }
-        }
-    };
-    int pc[9], pcn[9];
-    load_codes((long long)blockIdx.x * 128 + row, pc);
-
-    for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-        // ---- A operand: one-hot row of this thread's cell (row `row` of the tile), this thread's taps ----
-#pragma unroll
-        for (int t = 0; t < 9; t++) {
-            if (t < t_lo || t >= t_hi) continue;
-            const uint32_t one = 0x3C00u << ((pc[t] & 1) * 16);      // fp16 1.0 in the low or high half of a word
-            const int w = pc[t] >> 1;                                  // word 0..7 inside the 16-wide slot
-            uint4 lo, hi;
-            lo.x = w == 0 ? one : 0u; lo.y = w == 1 ? one : 0u; lo.z = w == 2 ? one : 0u; lo.w = w == 3 ? one : 0u;
-            hi.x = w == 4 ? one : 0u; hi.y = w == 5 ? one : 0u; hi.z = w == 6 ? one : 0u; hi.w = w == 7 ? one : 0u;
-            if (t == 4) hi.w |= 0x3C000000u;                           // slot 15 of the centre tap: constant 1 -> bias row of B
-            *reinterpret_cast<uint4 *>(rowp + (2 * t) * 2048) = lo;
-            *reinterpret_cast<uint4 *>(rowp + (2 * t + 1) * 2048) = hi;
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); // generic-proxy smem writes (A, and B on the first tile) -> visible to the tensor cores
-        __syncthreads();
-        float d[64];
-#pragma unroll
-        for (int i = 0; i < 64; i++) d[i] = 0.f;
-        wgmma_fence();
-#pragma unroll
-        for (int t = 0; t < 9; t++) Wgmma<128>::mma(d, da + (uint64_t)((t * 4096) >> 4), db + (uint64_t)((t * 4096) >> 4), 1u);   // two k-chunks per MMA
-        wgmma_commit();
-        load_codes((tile + gridDim.x) * 128 + row, pcn);             // next tile's board bytes fly while the tensor cores work
-        wgmma_wait<0>();
-        fence_regs(d);
-        // ---- epilogue: this warp owns tile rows rb .. rb+15 (lane: rows rb + lane/4 and + 8, channel pairs 8j + 2(lane%4)).  The fp16
-        // rows are staged in this warp's private slice of sOut with an XOR swizzle on the 16-byte chunk index (conflict-free), then
-        // written with fully coalesced 512-byte warp stores (two rows per instruction). ----
-        const int rb = wg * 64 + (warp & 3) * 16, q = lane & 3;
-#pragma unroll
-        for (int h = 0; h < 2; h++) {
-            const int r = rb + (lane >> 2) + 8 * h;
-#pragma unroll
-            for (int j = 0; j < 16; j++)
-                *reinterpret_cast<__half2 *>(sOut + r * 256 + ((j ^ (r & 15)) << 4) + q * 4) =
-                    __floats2half2_rn(fmaxf(d[4 * j + 2 * h], 0.f), fmaxf(d[4 * j + 2 * h + 1], 0.f));
-        }
-        __syncwarp();
-        {
-            const long long row0 = tile * 128 + rb;                    // first cell of this warp's 16 rows
-            const int half = lane >> 4, ch = lane & 15;
-#pragma unroll 4
-            for (int i = 0; i < 8; i++) {
-                const int r = 2 * i + half;
-                if (row0 + r < total) {
-                    const uint4 o = *reinterpret_cast<const uint4 *>(sOut + (rb + r) * 256 + ((ch ^ ((rb + r) & 15)) << 4));
-                    *reinterpret_cast<uint4 *>(out + (size_t)(row0 + r) * 128 + ch * 8) = o;
-                }
-            }
-        }
-        __syncthreads();                                               // every warpgroup's MMAs have read A before the next tile overwrites it
-#pragma unroll
-        for (int t = 0; t < 9; t++) pc[t] = pcn[t];
-    }
-}
-
-// ------------------------------------------------------------------------------------------
-// heads, stage 1: conv1x1 (128 -> 3) + bias + ReLU.  One CTA per position; all loads of a warp are issued first.
-// ------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_head_conv(const __half *__restrict__ x /* [B][90][128] */, int B, const float *__restrict__ wh /* [3][128] */,
-                                                    const float *__restrict__ bh /* [3] */, __half *__restrict__ hp /* [B][192] */,
-                                                    float *__restrict__ hv /* [B][96] */) {
-    const int pos = blockIdx.x;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int half_id = lane >> 4, l16 = lane & 15;   // two cells per warp iteration, 16 lanes x 8 channels each
-    float wreg[3][8];
-#pragma unroll
-    for (int o = 0; o < 3; o++)
-#pragma unroll
-        for (int k = 0; k < 8; k++) wreg[o][k] = __ldg(wh + o * 128 + l16 * 8 + k);
-    const float bh0 = bh[0], bh1 = bh[1], bh2 = bh[2];
-    uint4 raw[6];
-#pragma unroll
-    for (int j = 0; j < 6; j++) {                     // cells: (warp + 8j)*2 + half_id, 45 pairs over 8 warps
-        const int cell = (warp + 8 * j) * 2 + half_id;
-        raw[j] = cell < 90 ? __ldg(reinterpret_cast<const uint4 *>(x + ((size_t)pos * 90 + cell) * 128 + l16 * 8)) : make_uint4(0, 0, 0, 0);
-    }
-#pragma unroll
-    for (int j = 0; j < 6; j++) {
-        const int cell = (warp + 8 * j) * 2 + half_id;
-        const __half2 *h2 = reinterpret_cast<const __half2 *>(&raw[j]);
-        float s0 = 0.f, s1 = 0.f, s2 = 0.f;
-#pragma unroll
-        for (int k = 0; k < 4; k++) {
-            const float2 v = __half22float2(h2[k]);
-            s0 += v.x * wreg[0][2 * k] + v.y * wreg[0][2 * k + 1];
-            s1 += v.x * wreg[1][2 * k] + v.y * wreg[1][2 * k + 1];
-            s2 += v.x * wreg[2][2 * k] + v.y * wreg[2][2 * k + 1];
-        }
-#pragma unroll
-        for (int o = 8; o >= 1; o >>= 1) {
-            s0 += __shfl_xor_sync(0xffffffffu, s0, o);
-            s1 += __shfl_xor_sync(0xffffffffu, s1, o);
-            s2 += __shfl_xor_sync(0xffffffffu, s2, o);
-        }
-        if (l16 == 0 && cell < 90) {
-            // flatten order of tf.reshape on NHWC (policy_value_network.py:62, 72): index = cell*2 + c
-            *reinterpret_cast<__half2 *>(hp + (size_t)pos * 192 + cell * 2) = __floats2half2_rn(fmaxf(s0 + bh0, 0.f), fmaxf(s1 + bh1, 0.f));
-            hv[(size_t)pos * 96 + cell] = fmaxf(s2 + bh2, 0.f);
-        }
-    }
-    if (threadIdx.x < 12) hp[(size_t)pos * 192 + 180 + threadIdx.x] = __float2half(0.f);   // K padding of the policy GEMM
-}
-
 // heads, stage 2a: value MLP 90 -> 256 ReLU -> 1 tanh (policy_value_network.py:73-74), 8 positions per CTA.
 // Thread t owns hidden unit t: its 90 first-layer weights are requested up front (90 independent coalesced loads, one L2 round trip
 // instead of nine), the positions' features are broadcast from shared memory.
@@ -338,13 +119,8 @@ __global__ void __launch_bounds__(256) k_value_mlp(const float *__restrict__ hv 
 }
 
 // ------------------------------------------------------------------------------------------
-// heads, stage 2b: policy FC on tensor cores (legacy mma.sync path: 0.77 GFLOP, bound by its 8.5 MB f32 output)
-// ------------------------------------------------------------------------------------------
-
-// ------------------------------------------------------------------------------------------
-// heads, stage 1 on the (legacy) tensor path: the same conv1x1 (128 -> 3) as one streaming pass.
-// k_head_conv above spends 5.5 M warp instructions on shuffles and conversions to read 23.6 MB (13 us, 22 % of DRAM peak).  Here a CTA
-// (one position, 6 warps) stages its 90 x 128 fp16 cells in shared memory with cp.async (rows padded to 272 B: conflict-free
+// heads, stage 1: conv1x1 (128 -> 3) + bias + ReLU as one streaming pass.
+// A CTA (one position, 6 warps) stages its 90 x 128 fp16 cells in shared memory with cp.async (rows padded to 272 B: conflict-free
 // ldmatrix), each warp multiplies its 16 cells with mma.sync m16n8k16 against the head weights held in registers as B fragments
 // (N = 8: policy 2 + value 1 + 5 zero columns).  The f32 weights enter as hi + lo fp16 pairs (two MMAs per k-step), so the result
 // equals the fp32-weight dot product to ~1e-7 relative: no precision is traded for the speed.  ~2 instructions per cell.
@@ -497,6 +273,8 @@ __global__ void __launch_bounds__(256) k_policy_fc_tc(const uint4 *__restrict__ 
 constexpr int NPAD = 2112;   // 33 * 64 >= 2086
 constexpr int LDS_ROW = 200; // halves per staged row (192 + 8 pad): fragment loads hit 32 distinct banks
 
+// ------------------------------------------------------------------------------------------
+// heads, stage 2b for smaller batches: the policy FC on mma.sync m16n8k16 (0.77 GFLOP at 1024 positions, bound by its 8.5 MB f32 output)
 // grid (ceil(B/64), 33), 128 threads.  A tile (64 positions x 192) and B tile (64 labels x 192) are staged through shared
 // memory with 16-byte coalesced loads, all in flight at once; warp w owns rows [16w, 16w+16) x 64 columns.
 __global__ void __launch_bounds__(128) k_policy_fc(const __half *__restrict__ hp /* [B][192] */, int B, const __half *__restrict__ wp /* [NPAD][192] */,
@@ -554,29 +332,9 @@ __global__ void __launch_bounds__(128) k_policy_fc(const __half *__restrict__ hp
 //      fp16's range: |hi| <= 65504, residues below 2^-24 * 2^11 flush).
 // A TF32 convolution hi(x) * hi(w) (K = 1152: the only long accumulation chain of full-size terms) plus an fp16 convolution
 // x2 * { hi(w) | lo(w) * 2^11 } (the two cross terms, 2^-11 smaller, scaled back by 2^-11 in the epilogue) give the product to
-// O(2^-22): dropped are lo*lo and the 11-bit rounding of the two lo operands.  Streaming kernel: 32 B in, 64 B out per thread.
+// O(2^-22): dropped are lo*lo and the 11-bit rounding of the two lo operands.
 __device__ __forceinline__ float tf32_hi(float v) { return __uint_as_float((__float_as_uint(v) + 0x1000u) & 0xFFFFE000u); }
 #define SPLIT_SCALE 2048.0f
-
-__global__ void __launch_bounds__(256) k_split_tf32(const float4 *__restrict__ y, float4 *__restrict__ hi, uint4 *__restrict__ x2, long long n8) {
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n8; i += (long long)gridDim.x * blockDim.x) {
-        const float4 a = __ldg(y + 2 * i), b = __ldg(y + 2 * i + 1);
-        const float4 ha = make_float4(tf32_hi(a.x), tf32_hi(a.y), tf32_hi(a.z), tf32_hi(a.w));
-        const float4 hb = make_float4(tf32_hi(b.x), tf32_hi(b.y), tf32_hi(b.z), tf32_hi(b.w));
-        hi[2 * i] = ha; hi[2 * i + 1] = hb;
-        uint4 l, h;
-        *reinterpret_cast<__half2 *>(&l.x) = __floats2half2_rn((a.x - ha.x) * SPLIT_SCALE, (a.y - ha.y) * SPLIT_SCALE);
-        *reinterpret_cast<__half2 *>(&l.y) = __floats2half2_rn((a.z - ha.z) * SPLIT_SCALE, (a.w - ha.w) * SPLIT_SCALE);
-        *reinterpret_cast<__half2 *>(&l.z) = __floats2half2_rn((b.x - hb.x) * SPLIT_SCALE, (b.y - hb.y) * SPLIT_SCALE);
-        *reinterpret_cast<__half2 *>(&l.w) = __floats2half2_rn((b.z - hb.z) * SPLIT_SCALE, (b.w - hb.w) * SPLIT_SCALE);
-        *reinterpret_cast<__half2 *>(&h.x) = __floats2half2_rn(ha.x, ha.y);
-        *reinterpret_cast<__half2 *>(&h.y) = __floats2half2_rn(ha.z, ha.w);
-        *reinterpret_cast<__half2 *>(&h.z) = __floats2half2_rn(hb.x, hb.y);
-        *reinterpret_cast<__half2 *>(&h.w) = __floats2half2_rn(hb.z, hb.w);
-        uint4 *o = x2 + (i >> 4) * 32 + (i & 15);          // row of 256 halves = 32 uint4: { lo: 16 | hi: 16 }
-        o[0] = l; o[16] = h;
-    }
-}
 
 // One pass per convolution: v = ReLU(t + 2^-11 s + bias [+ skip]) from the two library convolutions' raw results, then the split of v
 // for the NEXT convolution.  t f32 [P][128] (hi*hi), s fp16 [P][128] or null (cross terms, scaled), skip f32 or null; outputs (each
@@ -623,6 +381,33 @@ __global__ void __launch_bounds__(256) k_epilogue_split(const float4 *__restrict
     }
 }
 
+// The value MLP and the policy FC are independent: fork the value MLP onto a side stream (event fork/join, which CUDA-graph
+// capture records as two parallel branches) so that the two small kernels overlap.  launch_policy_fc(st) launches the policy FC
+// on the caller's stream between the fork and the join.  The side stream and its events are created on the first (eager,
+// warm-up) call of either heads entry point, never during capture.
+template <class LaunchPolicyFc>
+int value_mlp_beside(cudaStream_t st, const float *hv, int B, const float *w1t, const float *b1, const float *w2, const float *b2, float *value,
+                     LaunchPolicyFc launch_policy_fc) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return CZ_ECUDA;
+    static cudaStream_t side[64] = {nullptr};
+    static cudaEvent_t ev_fork[64] = {nullptr}, ev_join[64] = {nullptr};
+    if (!side[dev]) {
+        if (cudaStreamCreateWithFlags(&side[dev], cudaStreamNonBlocking) != cudaSuccess) return CZ_ECUDA;
+        if (cudaEventCreateWithFlags(&ev_fork[dev], cudaEventDisableTiming) != cudaSuccess) return CZ_ECUDA;
+        if (cudaEventCreateWithFlags(&ev_join[dev], cudaEventDisableTiming) != cudaSuccess) return CZ_ECUDA;
+    }
+    if (cudaEventRecord(ev_fork[dev], st) != cudaSuccess) return CZ_ECUDA;
+    if (cudaStreamWaitEvent(side[dev], ev_fork[dev], 0) != cudaSuccess) return CZ_ECUDA;
+    k_value_mlp<<<(B + VM_POS - 1) / VM_POS, 256, 0, side[dev]>>>(hv, B, w1t, b1, w2, b2, value);
+    if (cudaGetLastError() != cudaSuccess) return CZ_ECUDA;
+    if (cudaEventRecord(ev_join[dev], side[dev]) != cudaSuccess) return CZ_ECUDA;
+    launch_policy_fc(st);
+    if (cudaGetLastError() != cudaSuccess) return CZ_ECUDA;
+    if (cudaStreamWaitEvent(st, ev_join[dev], 0) != cudaSuccess) return CZ_ECUDA;
+    return CZ_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -634,27 +419,6 @@ int cz_net_first_conv(const uint8_t *canon_boards, int B, const void *w1, const 
     return cudaGetLastError() == cudaSuccess ? CZ_OK : CZ_ECUDA;
 }
 
-int cz_net_first_conv_mma(const uint8_t *canon_boards, int B, const void *w_frag, void *out, void *stream) {
-    if (!canon_boards || !w_frag || !out || B <= 0) return CZ_EINVAL;
-    k_first_conv_mma<<<(B + FCM_POS - 1) / FCM_POS, 256, 0, (cudaStream_t)stream>>>(canon_boards, B, reinterpret_cast<const uint2 *>(w_frag),
-                                                                                     reinterpret_cast<__half *>(out));
-    return cudaGetLastError() == cudaSuccess ? CZ_OK : CZ_ECUDA;
-}
-
-int cz_net_first_conv_tc(const uint8_t *canon_boards, int B, const void *w_umma, const float *b1, void *out, void *stream) {
-    if (!canon_boards || !w_umma || !b1 || !out || B <= 0) return CZ_EINVAL;
-    const int smem = 2 * TC_TILE_BYTES + TC_OUT_BYTES;   // 106 496 B > 48 KB default: opt in
-    if (cudaFuncSetAttribute(k_first_conv_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) return CZ_ECUDA;
-    const long long tiles = ((long long)B * 90 + 127) / 128;
-    int dev = 0, sms = 132;
-    if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const long long grid = tiles < sms ? tiles : sms;                // persistent: one CTA per SM
-    (void)b1;                                                         // the bias is row (centre tap, slot 15) of w_umma
-    k_first_conv_tc<<<(unsigned)grid, 256, smem, (cudaStream_t)stream>>>(canon_boards, B, reinterpret_cast<const uint4 *>(w_umma),
-                                                                        reinterpret_cast<__half *>(out));
-    return cudaGetLastError() == cudaSuccess ? CZ_OK : CZ_ECUDA;
-}
-
 // value MLP (side stream) || policy FC on already computed head features hp / hv
 int cz_net_heads_fc(const void *hp, const float *hv, int B, const float *w1t, const float *b1, const float *w2, const float *b2,
                     const void *wp, const float *bp, float *logits, float *value, void *stream) {
@@ -662,39 +426,18 @@ int cz_net_heads_fc(const void *hp, const float *hv, int B, const float *w1t, co
     cudaStream_t st = (cudaStream_t)stream;
     const int smem = 2 * 64 * LDS_ROW * (int)sizeof(__half);   // 51200 B > the 48 KB default: opt in (per device, so every call)
     if (cudaFuncSetAttribute(k_policy_fc, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) return CZ_ECUDA;
-    // The value MLP and the policy FC are independent: fork the value MLP onto a side stream (event fork/join, which
-    // CUDA-graph capture records as two parallel branches) so that the two small kernels overlap.
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return CZ_ECUDA;
-    static cudaStream_t side[64] = {nullptr};
-    static cudaEvent_t ev_fork[64] = {nullptr}, ev_join[64] = {nullptr};
-    if (!side[dev]) {   // created on the first (eager, warm-up) call, never during capture
-        if (cudaStreamCreateWithFlags(&side[dev], cudaStreamNonBlocking) != cudaSuccess) return CZ_ECUDA;
-        if (cudaEventCreateWithFlags(&ev_fork[dev], cudaEventDisableTiming) != cudaSuccess) return CZ_ECUDA;
-        if (cudaEventCreateWithFlags(&ev_join[dev], cudaEventDisableTiming) != cudaSuccess) return CZ_ECUDA;
-    }
-    if (cudaEventRecord(ev_fork[dev], st) != cudaSuccess) return CZ_ECUDA;
-    if (cudaStreamWaitEvent(side[dev], ev_fork[dev], 0) != cudaSuccess) return CZ_ECUDA;
-    k_value_mlp<<<(B + VM_POS - 1) / VM_POS, 256, 0, side[dev]>>>(hv, B, w1t, b1, w2, b2, value);
-    if (cudaGetLastError() != cudaSuccess) return CZ_ECUDA;
-    if (cudaEventRecord(ev_join[dev], side[dev]) != cudaSuccess) return CZ_ECUDA;
-    dim3 grid((B + 63) / 64, NPAD / 64);
-    k_policy_fc<<<grid, 128, smem, st>>>((const __half *)hp, B, (const __half *)wp, bp, logits);
-    if (cudaGetLastError() != cudaSuccess) return CZ_ECUDA;
-    if (cudaStreamWaitEvent(st, ev_join[dev], 0) != cudaSuccess) return CZ_ECUDA;
-    return CZ_OK;
+    return value_mlp_beside(st, hv, B, w1t, b1, w2, b2, value, [&](cudaStream_t s) {
+        k_policy_fc<<<dim3((B + 63) / 64, NPAD / 64), 128, smem, s>>>((const __half *)hp, B, (const __half *)wp, bp, logits);
+    });
 }
 
 int cz_net_heads(const void *x, int B, const float *wh, const float *bh, const float *w1t, const float *b1, const float *w2, const float *b2,
                  const void *wp, const float *bp, void *hp_scratch, float *hv_scratch, float *logits, float *value, void *stream) {
     if (!x || !wh || !bh || !hp_scratch || !hv_scratch || B <= 0) return CZ_EINVAL;
-    static const bool legacy = getenv("CCHESS_HEAD_CONV") && !strcmp(getenv("CCHESS_HEAD_CONV"), "simt");
-    if (legacy) k_head_conv<<<B, 256, 0, (cudaStream_t)stream>>>((const __half *)x, B, wh, bh, (__half *)hp_scratch, hv_scratch);
-    else k_head_conv_mma<false><<<B, 192, 0, (cudaStream_t)stream>>>((const __half *)x, B, wh, bh, (__half *)hp_scratch, hv_scratch);
+    k_head_conv_mma<false><<<B, 192, 0, (cudaStream_t)stream>>>((const __half *)x, B, wh, bh, (__half *)hp_scratch, hv_scratch);
     if (cudaGetLastError() != cudaSuccess) return CZ_ECUDA;
     return cz_net_heads_fc(hp_scratch, hv_scratch, B, w1t, b1, w2, b2, wp, bp, logits, value, stream);
 }
-
 
 // The heads for large batches: conv1x1 on mma.sync writing the policy features in the wgmma-tiled layout, value MLP on a side stream,
 // policy FC on wgmma (k_policy_fc_tc).  wp_tiled: dev fp16 [17 label tiles][24 k-chunks][128 labels][8] (labels >= 2086 zero),
@@ -707,42 +450,14 @@ int cz_net_heads_tc(const void *x, int B, const float *wh, const float *bh, cons
     if (cudaFuncSetAttribute(k_policy_fc_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) return CZ_ECUDA;
     k_head_conv_mma<true><<<B, 192, 0, st>>>((const __half *)x, B, wh, bh, (__half *)hp_tiled_scratch, hv_scratch);
     if (cudaGetLastError() != cudaSuccess) return CZ_ECUDA;
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return CZ_ECUDA;
-    static cudaStream_t side[64] = {nullptr};
-    static cudaEvent_t ev_fork[64] = {nullptr}, ev_join[64] = {nullptr};
-    if (!side[dev]) {   // created on the first (eager, warm-up) call, never during capture
-        if (cudaStreamCreateWithFlags(&side[dev], cudaStreamNonBlocking) != cudaSuccess) return CZ_ECUDA;
-        if (cudaEventCreateWithFlags(&ev_fork[dev], cudaEventDisableTiming) != cudaSuccess) return CZ_ECUDA;
-        if (cudaEventCreateWithFlags(&ev_join[dev], cudaEventDisableTiming) != cudaSuccess) return CZ_ECUDA;
-    }
-    if (cudaEventRecord(ev_fork[dev], st) != cudaSuccess) return CZ_ECUDA;
-    if (cudaStreamWaitEvent(side[dev], ev_fork[dev], 0) != cudaSuccess) return CZ_ECUDA;
-    k_value_mlp<<<(B + VM_POS - 1) / VM_POS, 256, 0, side[dev]>>>(hv_scratch, B, w1t, b1, w2, b2, value);
-    if (cudaGetLastError() != cudaSuccess) return CZ_ECUDA;
-    if (cudaEventRecord(ev_join[dev], side[dev]) != cudaSuccess) return CZ_ECUDA;
-    dim3 grid((B + 127) / 128, 17);
-    k_policy_fc_tc<<<grid, 256, smem, st>>>((const uint4 *)hp_tiled_scratch, B, (const uint4 *)wp_tiled, bp, logits);
-    if (cudaGetLastError() != cudaSuccess) return CZ_ECUDA;
-    if (cudaStreamWaitEvent(st, ev_join[dev], 0) != cudaSuccess) return CZ_ECUDA;
-    return CZ_OK;
-}
-
-// y dev f32 [n_pix][128] -> hi dev f32 [n_pix][128] = tf32(y), x2 dev fp16 [n_pix][256] = { (y - hi) * 2^11 | hi } (see k_split_tf32)
-int cz_net_split_tf32(const float *y, float *hi, void *x2, long long n_pix, void *stream) {
-    if (!y || !hi || !x2 || n_pix <= 0) return CZ_EINVAL;
-    const long long n8 = n_pix * 16;
-    int dev = 0, sms = 132;
-    if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    long long blocks = (n8 + 255) / 256;
-    if (blocks > 8LL * sms) blocks = 8LL * sms;          // grid-stride, 8 resident CTAs of 256 threads per SM
-    k_split_tf32<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const float4 *>(y), reinterpret_cast<float4 *>(hi),
-                                                                    reinterpret_cast<uint4 *>(x2), n8);
-    return cudaGetLastError() == cudaSuccess ? CZ_OK : CZ_ECUDA;
+    return value_mlp_beside(st, hv_scratch, B, w1t, b1, w2, b2, value, [&](cudaStream_t s) {
+        k_policy_fc_tc<<<dim3((B + 127) / 128, 17), 256, smem, s>>>((const uint4 *)hp_tiled_scratch, B, (const uint4 *)wp_tiled, bp, logits);
+    });
 }
 
 // The f32 epilogue of one three-product convolution fused with the operand split for the next one (k_epilogue_split):
-//   v = ReLU(t + 2^-11 s + bias [+ skip]);  x (optional) = v;  hi / x2 (optional, both or neither) = split of v as in cz_net_split_tf32.
+//   v = ReLU(t + 2^-11 s + bias [+ skip]);  x (optional) = v;  hi / x2 (optional, both or neither) = split of v
+//   (hi = tf32(v), x2 = { (v - hi) * 2^11 | hi }, see above).
 // t dev f32 [n_pix][128]; s dev fp16 [n_pix][128] or NULL; bias dev f32 [128]; skip dev f32 [n_pix][128] or NULL (x may alias skip).
 int cz_net_epilogue_split(const float *t, const void *s, const float *bias, const float *skip, float *x, float *hi, void *x2, long long n_pix, void *stream) {
     if (!t || !bias || n_pix <= 0 || (!x && !hi) || ((hi == nullptr) != (x2 == nullptr))) return CZ_EINVAL;

@@ -6,10 +6,10 @@
 // the library path is 15+ launches of ~5 us each, every one re-reading its weights; here the activations of a position never
 // leave the SMs and the weights stream from L2 under the tensor cores.
 //
-// Shape: one thread-block CLUSTER of CL CTAs (CL = 1, 2, 4 or 8) per position; CTA r owns output channels
-// [r*128/CL, (r+1)*128/CL).  Per 3x3 convolution and CTA:
-//     D[128 rows][128/CL ch] (f32, registers) = sum over 9 taps of  A_tap[128][128] . B_tap[128][128/CL]
-//   as two warpgroups, each 72 wgmma.mma_async m64nNk16 over its 64 rows (N = 128/CL).
+// Shape: one thread-block CLUSTER of CL = 4 CTAs per position; CTA r owns output channels [r*NC, (r+1)*NC), NC = 128/CL = 32.
+// Per 3x3 convolution and CTA:
+//     D[128 rows][NC ch] (f32, registers) = sum over 9 taps of  A_tap[128][128] . B_tap[128][NC]
+//   as two warpgroups, each 72 wgmma.mma_async m64n32k16 over its 64 rows.
 //   * A = the position's activation image, fp16, resident in shared memory in the canonical K-major NO-SWIZZLE layout
 //     [16 k-chunks of 8 channels][152 rows][8 halves]: with SBO = 128 B consecutive rows are 16 bytes apart in every chunk, so a
 //     3x3 tap is nothing but a START-ADDRESS OFFSET of (dr*11 + df) rows in the A descriptor -- no im2col, no copies.  Rows are
@@ -18,17 +18,14 @@
 //   * B = this CTA's slice of the layer's weights, streamed tap by tap from L2 by TMA (cp.async.bulk.tensor, SASS UTMALDG)
 //     through a ring of shared-memory stages (full / empty mbarriers); the producer runs ahead across layers.
 //   * epilogue: each math thread adds bias (+ the residual skip) to its accumulator fragment, applies ReLU, converts to fp16 and
-//     writes its channel pairs of the NEXT layer's A image into the shared memory of ALL CL CTAs of the cluster (DSMEM stores);
-//     a CTA starts the next layer when all CL CTAs' slices have arrived on its `act_ready` mbarrier.  No cluster-wide barrier on
-//     the critical path.
+//     writes its channel pairs of the NEXT layer's A image into the shared memory of ALL CL CTAs of the cluster (st.async DSMEM
+//     stores that complete their byte count on the receiver's `act_ready` mbarrier); a CTA starts the next layer when all bytes of
+//     the image have arrived.  No cluster-wide barrier on the critical path.
 // Warp roles: 8 math warps (two warpgroups: MMA rows 0-63 and 64-127), then one TMA producer warp (one elected lane).
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
-#include <stdio.h>
-#include <stdlib.h>
-#include <string.h>
 
 #include "../../include/cchess_b200.h"
 #include "cz_wgmma.cuh"
@@ -44,6 +41,10 @@ constexpr int A_BYTES = 16 * LBO_A;       // 38 912 B per activation image
 constexpr int NMATH = 256;                // two warpgroups
 constexpr int NMATH_WARPS = NMATH / 32;
 constexpr int NTHREADS = NMATH + 32;      // + the TMA producer warp
+constexpr int CL = 4;                     // CTAs per cluster (one position)
+constexpr int NC = 128 / CL;              // output channels of one CTA (= wgmma N)
+constexpr int STAGE_BYTES = NC * 256;     // one tap of a CTA's weight slice: [16 k-chunks][NC rows][8 halves]
+constexpr int S = 16;                     // weight ring depth (stages)
 
 // Byte offset of (8-channel chunk 0..15, raster row) inside an activation image: canonical K-major NO-SWIZZLE layout
 // [16 chunks][ROWS rows][16 B] (LBO = ROWS*16, SBO = 128).  A tap shift is a start-address offset of whole rows.
@@ -71,33 +72,6 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t *b, uint32_t bytes) {
 }
 __device__ __forceinline__ void mbar_arrive(uint64_t *b) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(b)) : "memory");
-}
-// relaxed arrive on the barrier at the same shared-memory offset in CTA `rank`; the caller has issued fence.acq_rel.cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t *b, uint32_t rank) {
-    uint32_t ra;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(smem_u32(b)), "r"(rank));
-    asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(ra) : "memory");
-}
-// publish this warp's image writes (generic proxy, local + remote shared memory) and signal every CTA of the cluster
-template <int CL>
-__device__ __forceinline__ void publish_image(uint64_t *bar, int lane) {
-    asm volatile("fence.proxy.async;" ::: "memory");                     // generic-proxy writes -> visible to the tensor cores (async proxy)
-    __syncwarp();
-    if (lane == 0) {
-        if (CL > 1) asm volatile("fence.acq_rel.cluster;" ::: "memory"); // one release for the whole warp's stores
-#pragma unroll
-        for (int q = 0; q < CL; q++) mbar_arrive_remote(bar, (uint32_t)q);
-    }
-}
-__device__ __forceinline__ void st_cluster_v4(uint32_t local_addr, uint32_t rank, uint4 v) {
-    uint32_t ra;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(local_addr), "r"(rank));
-    asm volatile("st.shared::cluster.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(ra), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-__device__ __forceinline__ void st_cluster_b32(uint32_t local_addr, uint32_t rank, uint32_t v) {
-    uint32_t ra;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(local_addr), "r"(rank));
-    asm volatile("st.shared::cluster.b32 [%0], %1;" ::"r"(ra), "r"(v) : "memory");
 }
 // Async-proxy stores into CTA `rank`'s shared memory that complete their byte count on THAT CTA's mbarrier: the designed
 // DSMEM producer -> consumer path.  The barrier completes by byte count: no arrive loop, no release fence on the critical path.
@@ -134,25 +108,19 @@ struct TowerArgs {
     float *hv;                 // out [n][96]
     int n_pos;
     int n_conv;                // 2 * res_block_nums
-    long long *trace;          // optional (CCHESS_TOWER_TRACE): clock64 stamps of position 0 / CTA 0, 8 per layer
 };
 
-// ASYNC_ST: image slices travel by st.async (complete_tx on the receiver's barrier) instead of generic stores + proxy fence + arrives.
-template <int CL, bool ASYNC_ST>
 __global__ void __launch_bounds__(NTHREADS, 1) k_tower_small(const __grid_constant__ CUtensorMap wmap, TowerArgs a) {
     constexpr uint32_t IMAGE_TX = 128u * 16u * 16u;        // bytes every CTA receives per image: 128 rows x 16 chunks x 16 B
-    constexpr int NC = 128 / CL;                           // output channels of this CTA (= wgmma N)
     constexpr int W = NC / 2;                              // layer 0: channels per math thread (two column groups)
     static_assert(W % 8 == 0 && W >= 8, "layer-0 column groups");
-    constexpr int STAGE_BYTES = NC * 256;                  // one tap of this CTA's weight slice: [16 k-chunks][NC rows][8 halves]
-    constexpr int S = CL == 1 ? 4 : (CL == 2 ? 8 : 16);    // ring depth
     extern __shared__ __align__(128) unsigned char smem[];
     unsigned char *bufX = smem, *bufY = smem + A_BYTES, *ring = smem + 2 * A_BYTES;
     float *s_bias = reinterpret_cast<float *>(ring + S * STAGE_BYTES);      // [n_layers][NC] this CTA's slice
     __shared__ __align__(8) uint64_t full[S], empty[S], act_ready[2];       // act_ready ping-pongs by layer parity: arrivals of consecutive layers never mix
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const uint32_t rank = CL == 1 ? 0u : cluster_rank();
+    const uint32_t rank = cluster_rank();
     const int pos = blockIdx.x / CL;
     const int n_layers = 1 + a.n_conv;
 
@@ -161,13 +129,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_tower_small(const __grid_consta
     for (int i = tid; i < n_layers * NC; i += NTHREADS) s_bias[i] = a.bias[(i / NC) * 128 + rank * NC + (i % NC)];
     if (tid == 0) {
         for (int s = 0; s < S; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], NMATH_WARPS); }
-        mbar_init(&act_ready[0], ASYNC_ST ? 1 : CL * NMATH_WARPS);      // ASYNC_ST: one arrive.expect_tx by thread 0 + IMAGE_TX bytes
-        mbar_init(&act_ready[1], ASYNC_ST ? 1 : CL * NMATH_WARPS);
+        mbar_init(&act_ready[0], 1);                     // one arrive.expect_tx by thread 0 + IMAGE_TX bytes
+        mbar_init(&act_ready[1], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     asm volatile("fence.proxy.async;" ::: "memory");     // the zeroed images (generic proxy) are what the tensor cores will read as padding
     __syncthreads();
-    if (CL > 1) cluster_sync_all();                      // every CTA's barriers and zeroed images exist before anyone writes remotely
+    cluster_sync_all();                                  // every CTA's barriers and zeroed images exist before anyone writes remotely
 
     if (warp == NMATH_WARPS) {
         // ===== TMA producer: taps of all layers, in order, as fast as the ring frees up =====
@@ -229,12 +197,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_tower_small(const __grid_consta
 #pragma unroll
                 for (int qi = 0; qi < CL; qi++) {
                     const uint32_t q = (rank + 1u + (uint32_t)qi) & (uint32_t)(CL - 1);   // every CTA starts with a different receiver (ingress spread), itself last
-                    if (ASYNC_ST) st_async_v4(dst, smem_u32(&act_ready[0]), (uint32_t)q, o);
-                    else if (CL == 1) *reinterpret_cast<uint4 *>(bufX + img_off(chunk, P0 + j)) = o;
-                    else st_cluster_v4(dst, (uint32_t)q, o);
+                    st_async_v4(dst, smem_u32(&act_ready[0]), q, o);
                 }
             }
-            if (!ASYNC_ST) publish_image<CL>(&act_ready[0], lane);                // image 0
         }
         // ===== residual tower: warpgroup wg multiplies MMA rows [64 wg, 64 wg + 64); this thread's accumulator rows are j0, j0 + 8 =====
         const int wg = tid >> 7, q = lane & 3;
@@ -249,18 +214,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_tower_small(const __grid_consta
         int stage = 0;
         uint32_t phase = 0;
         for (int L = 0; L < a.n_conv; L++) {
-            const bool tr = a.trace && blockIdx.x == 0 && tid == 0;
             if (tid == 0) {
-                if (ASYNC_ST) mbar_expect_tx(&act_ready[L & 1], IMAGE_TX);      // our arrival + the byte count of image L
+                mbar_expect_tx(&act_ready[L & 1], IMAGE_TX);                    // our arrival + the byte count of image L
                 mbar_wait_cluster(&act_ready[L & 1], (uint32_t)((L >> 1) & 1));   // image L (this layer's input) is complete in OUR shared memory
             }
             math_sync();
-            if (tr) a.trace[L * 8 + 0] = clock64();
             const uint32_t abase = smem_u32((L & 1) ? bufY : bufX) + (uint32_t)((P0 + wg * 64) * 16);   // conv1 of a block reads X, conv2 reads Y
             int prev = 0;
             for (int t = 0; t < 9; t++) {
                 mbar_wait(&full[stage], phase);
-                if (tr && t == 0) a.trace[L * 8 + 1] = clock64();
                 const int shift = (t / 3 - 1) * 11 + (t % 3 - 1);                // tap (dr, df) = a row offset in the padded raster
                 // Descriptors of the 8 K16 steps differ only in the start-address field: one add each from the tap's base descriptor.
                 const uint64_t da0 = gmma_desc(abase + (uint32_t)(shift * 16), LBO_A);
@@ -280,7 +242,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_tower_small(const __grid_consta
             wgmma_wait<0>();
             fence_regs(d);
             if (lane == 0) mbar_arrive(&empty[prev]);
-            if (tr) a.trace[L * 8 + 2] = a.trace[L * 8 + 3] = a.trace[L * 8 + 4] = clock64();
             // ---- epilogue: bias (+ skip), ReLU, fp16, this thread's channel pairs of image L + 1 into every CTA of the cluster ----
             const bool second = L & 1;                        // conv2 of a block: + skip (the block input, still in X), result back into X
             unsigned char *dstbuf = second ? bufX : bufY;
@@ -299,24 +260,16 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_tower_small(const __grid_consta
                     }
                     const __half2 o = cell[h] ? __floats2half2_rn(fmaxf(f0, 0.f), fmaxf(f1, 0.f)) : __floats2half2_rn(0.f, 0.f);
                     const uint32_t ov = *reinterpret_cast<const uint32_t *>(&o);
-                    if (ASYNC_ST) {
 #pragma unroll
-                        for (int qi = 0; qi < CL; qi++)   // receivers in rotated order: at any moment the CL senders address CL different CTAs
-                            st_async_b32(smem_u32(dstbuf) + off, smem_u32(&act_ready[(L + 1) & 1]), (rank + 1u + (uint32_t)qi) & (uint32_t)(CL - 1), ov);
-                    } else if (CL == 1) *reinterpret_cast<uint32_t *>(dstbuf + off) = ov;
-                    else {
-#pragma unroll
-                        for (int r = 0; r < CL; r++) st_cluster_b32(smem_u32(dstbuf) + off, (uint32_t)r, ov);
-                    }
+                    for (int qi = 0; qi < CL; qi++)   // receivers in rotated order: at any moment the CL senders address CL different CTAs
+                        st_async_b32(smem_u32(dstbuf) + off, smem_u32(&act_ready[(L + 1) & 1]), (rank + 1u + (uint32_t)qi) & (uint32_t)(CL - 1), ov);
                 }
             }
-            if (tr) a.trace[L * 8 + 5] = clock64();
-            if (!ASYNC_ST) publish_image<CL>(&act_ready[(L + 1) & 1], lane);       // image L + 1
         }
         // ---- heads: conv1x1 (128 -> 2 policy + 1 value) + bias + ReLU on the final image (in X), CTA 0 writes ----
         {
             if (tid == 0) {
-                if (ASYNC_ST) mbar_expect_tx(&act_ready[a.n_conv & 1], IMAGE_TX);
+                mbar_expect_tx(&act_ready[a.n_conv & 1], IMAGE_TX);
                 mbar_wait_cluster(&act_ready[a.n_conv & 1], (uint32_t)((a.n_conv >> 1) & 1));                // the final image (index n_conv) is complete
             }
             math_sync();                                                           // ordered behind thread 0's cluster-scope acquire
@@ -345,7 +298,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_tower_small(const __grid_consta
     }
     // ---- teardown: nobody leaves while a peer may still write into its shared memory ----
     __syncthreads();
-    if (CL > 1) cluster_sync_all();
+    cluster_sync_all();
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *, const cuuint32_t *,
@@ -362,80 +315,44 @@ EncodeTiledFn encode_tiled() {
     return fn;
 }
 
-template <int CL, bool ASYNC_ST>
-int launch_tower(const CUtensorMap &map, const TowerArgs &a, cudaStream_t st) {
-    constexpr int NC = 128 / CL, S = CL == 1 ? 4 : (CL == 2 ? 8 : 16);
-    const int n_layers = 1 + a.n_conv;
-    const size_t smem = 2 * (size_t)A_BYTES + (size_t)S * NC * 256 + (size_t)n_layers * NC * 4;
-    if (cudaFuncSetAttribute(k_tower_small<CL, ASYNC_ST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return CZ_ECUDA;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)(a.n_pos * CL));
-    cfg.blockDim = dim3(NTHREADS);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = CL; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, k_tower_small<CL, ASYNC_ST>, map, a) == cudaSuccess ? CZ_OK : CZ_ECUDA;
-}
-
 }  // namespace
 
 extern "C" {
 
-// Bytes of the weight blob cz_net_tower_small expects for `n_conv` 3x3 convolutions (independent of the cluster size).
+// Bytes of the weight blob cz_net_tower_small expects for `n_conv` 3x3 convolutions.
 int64_t cz_net_tower_blob_bytes(int n_conv) { return (int64_t)n_conv * 9 * 128 * 256; }
 
-int cz_net_tower_small(const uint8_t *canon_boards, int n_pos, int cluster, int n_conv, const void *w1, const void *wblob, const float *bias,
+int cz_net_tower_small(const uint8_t *canon_boards, int n_pos, int n_conv, const void *w1, const void *wblob, const float *bias,
                        const float *wh, const float *bh, void *hp, float *hv, void *stream) {
     if (!canon_boards || !w1 || !wblob || !bias || !wh || !bh || !hp || !hv || n_pos <= 0 || n_conv <= 0 || (n_conv & 1)) return CZ_EINVAL;
-    if (cluster != 1 && cluster != 2 && cluster != 4 && cluster != 8) return CZ_EINVAL;
     EncodeTiledFn enc = encode_tiled();
     if (!enc) return CZ_ECUDA;
     // the blob as a 2-D tensor of 256-byte rows: [n_conv * 9 * 128 rows][128 halves]; one box = one tap of one CTA's slice
     CUtensorMap map;
     const cuuint64_t gdim[2] = {128, (cuuint64_t)n_conv * 9 * 128};
     const cuuint64_t gstride[1] = {256};
-    const cuuint32_t box[2] = {128, (cuuint32_t)(128 / cluster)};
+    const cuuint32_t box[2] = {128, (cuuint32_t)NC};
     const cuuint32_t estr[2] = {1, 1};
     if (enc(&map, CU_TENSOR_MAP_DATA_TYPE_UINT16, 2, const_cast<void *>(wblob), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
             CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
         return CZ_ECUDA;
     TowerArgs a;
     a.boards = canon_boards; a.w1 = (const __half *)w1; a.bias = bias; a.wh = wh; a.bh = bh; a.hp = (__half *)hp; a.hv = hv;
-    a.n_pos = n_pos; a.n_conv = n_conv; a.trace = nullptr;
-    cudaStream_t st = (cudaStream_t)stream;
-    static const bool want_trace = getenv("CCHESS_TOWER_TRACE") != nullptr;       // debugging aid: per-layer clock64 stamps to stderr
-    static long long *trace_dev = nullptr;
-    static int trace_calls = 0;
-    if (want_trace) {
-        if (!trace_dev && cudaMalloc(&trace_dev, 64 * 8 * sizeof(long long)) != cudaSuccess) return CZ_ECUDA;
-        cudaMemsetAsync(trace_dev, 0, 64 * 8 * sizeof(long long), st);
-        a.trace = n_conv <= 62 ? trace_dev : nullptr;
-    }
-    struct TraceDump {
-        const TowerArgs &a; cudaStream_t st; long long *dev; int *calls;
-        ~TraceDump() {
-            if (!a.trace || ++*calls != 20) return;                               // one warm call, printed once
-            long long h[64 * 8];
-            cudaStreamSynchronize(st);
-            cudaMemcpy(h, dev, sizeof(h), cudaMemcpyDeviceToHost);
-            fprintf(stderr, "tower trace (clock64 deltas): layer: in_ready->w_ready, ->mma_issued, ->mma_done, ->(same), ->stores_issued, ->next in_ready\n");
-            for (int L = 0; L < a.n_conv; L++) {
-                const long long *r = h + L * 8, nxt = L + 1 < a.n_conv ? h[(L + 1) * 8] : r[5];
-                fprintf(stderr, "  L%02d: %6lld %6lld %6lld %6lld %6lld %6lld | layer %6lld\n", L, r[1] - r[0], r[2] - r[1], r[3] - r[2], r[4] - r[3], r[5] - r[4], nxt - r[5], nxt - r[0]);
-            }
-        }
-    } dump{a, st, trace_dev, &trace_calls};
-    static const bool generic_st = getenv("CCHESS_TOWER_ST") && !strcmp(getenv("CCHESS_TOWER_ST"), "generic");
-    switch (cluster) {
-        case 1: return generic_st ? launch_tower<1, false>(map, a, st) : launch_tower<1, true>(map, a, st);
-        case 2: return generic_st ? launch_tower<2, false>(map, a, st) : launch_tower<2, true>(map, a, st);
-        case 4: return generic_st ? launch_tower<4, false>(map, a, st) : launch_tower<4, true>(map, a, st);
-        default: return generic_st ? launch_tower<8, false>(map, a, st) : launch_tower<8, true>(map, a, st);
-    }
+    a.n_pos = n_pos; a.n_conv = n_conv;
+    const size_t smem = 2 * (size_t)A_BYTES + (size_t)S * STAGE_BYTES + (size_t)(1 + n_conv) * NC * 4;
+    if (cudaFuncSetAttribute(k_tower_small, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return CZ_ECUDA;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)(a.n_pos * CL));
+    cfg.blockDim = dim3(NTHREADS);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = (cudaStream_t)stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = CL; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, k_tower_small, map, a) == cudaSuccess ? CZ_OK : CZ_ECUDA;
 }
 
 }  // extern "C"
+

@@ -81,8 +81,8 @@ class MCTS_tree(object):
         if owner is not None and hasattr(owner, "native_plan") and getattr(owner, "precision", "") == "fp16":
             # the evaluator is this package's network: stay on the device (board bytes -> cz_net kernels -> tower) and
             # replay one CUDA graph per playout
-            # (<= 16 rows per call: the one-launch cluster trunk of csrc/cz_tower.cu; CCHESS_SMALL_TOWER=0 selects the library trunk)
-            small = K <= 16 and hasattr(owner, "small_plan") and os.environ.get("CCHESS_SMALL_TOWER", "1") != "0"
+            # (<= 16 rows per call: the one-launch cluster trunk of csrc/cz_tower.cu)
+            small = K <= 16 and hasattr(owner, "small_plan")
             self._plan = owner.small_plan(K) if small else owner.native_plan(K)
             self._nn_in = self._plan.make_input(K)
             self._dev_forward = lambda x, lo, v: self._plan(x, lo, v)

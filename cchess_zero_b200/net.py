@@ -98,7 +98,18 @@ def make_plan(net, precision, owner=None):
     return SplitTf32Plan(net, owner=owner) if precision == "tf32x3" else InferencePlan(net, precision, owner=owner)
 
 
-class InferencePlan:
+class _VersionedPlan:
+    """A plan that holds folded COPIES of its owner's weights.  policy_value_network.weights_version is bumped whenever the weights
+    change; refresh_if_stale re-derives the copies in place (`refresh`) when the plan's version is behind."""
+
+    def refresh_if_stale(self):
+        if self.owner is not None and self.owner.weights_version != self.version:
+            self.refresh()
+            return True
+        return False
+
+
+class InferencePlan(_VersionedPlan):
     """Eval-mode forward with batch norm folded into the convolutions, channels-last, in one of
     fp32 / tf32 / bf16 / fp16.  Takes the engine's NHWC batch as-is (its NCHW view is already
     channels_last) and returns float32 logits / value on the device."""
@@ -151,12 +162,6 @@ class InferencePlan:
                 for dst, src in zip(c1 + c2, n1 + n2):
                     dst.copy_(src)
         self.version = getattr(self.owner, "weights_version", self.version)
-
-    def refresh_if_stale(self):
-        if self.owner is not None and self.owner.weights_version != self.version:
-            self.refresh()
-            return True
-        return False
 
     def _probe_fused(self):
         try:
@@ -235,7 +240,7 @@ def split_weights(w):
 
 def split_acts(x):
     """[B, C, H, W] f32 -> (hi(x) f32 [B, C, H, W], { (x - hi(x)) * 2^11 | hi(x) } fp16 [B, 2C, H, W]): torch statement of
-    csrc/cz_net.cu: k_split_tf32."""
+    the split in csrc/cz_net.cu: k_epilogue_split."""
     h = tf32_hi(x)
     return h, torch.cat([(x - h) * SPLIT_SCALE, h], 1).to(torch.float16)
 
@@ -335,113 +340,102 @@ class SplitTf32Plan(InferencePlan):
         return logits, value
 
 
-class NativePlan:
-    """fp16 inference plan whose ends are the hand-written kernels of csrc/cz_net.cu:
-         board bytes --cz_net_first_conv--> [B,90,128] --library cuDNN convs (residual tower)--> --cz_net_heads--> logits, value
-    Input is the engine's CZ_BOARD output (uint8 [B,96], the side-to-move-canonical board); the one-hot
-    [9,10,14] tensor is never built.  Outputs are written straight into the float32 buffers the engine reads."""
+def _ends_weights(net, base):
+    """Kernel-layout copies of the weights both native plans share, derived from the folded fp16 base plan: the first convolution
+    (w1, fp16 [9 taps][14 pieces][128]), the 1x1 head convolutions (wh, bh), the value MLP (w1t, bv1, w2, b2t) and the zero-padded
+    policy FC (wp fp16 [2112][192], bp f32 [2112])."""
+    dev = base.w_in[0].device
+    with torch.no_grad():
+        w, _ = base.w_in                                                    # folded conv_in: [128,14,3,3] fp16
+        wh, bh = base.w_head                                                # [3,128,1,1]
+        wp = torch.zeros((2112, 192), dtype=torch.float16, device=dev)
+        wp[:NLABEL, :180] = net.p_fc.weight.detach().to(torch.float16)
+        bp = torch.zeros((2112,), dtype=torch.float32, device=dev)
+        bp[:NLABEL] = net.p_fc.bias.detach().float()
+        return dict(w1=w.float().permute(2, 3, 1, 0).reshape(9, 14, 128).to(torch.float16).contiguous(),
+                    wh=wh.float().reshape(3, 128).contiguous(), bh=bh.float().contiguous(),
+                    w1t=net.v_fc1.weight.detach().float().t().contiguous(),        # [90,256]
+                    bv1=net.v_fc1.bias.detach().float().contiguous(),
+                    w2=net.v_fc2.weight.detach().float().reshape(256).contiguous(),
+                    b2t=net.v_fc2.bias.detach().float().reshape(1).contiguous(), wp=wp, bp=bp)
+
+
+class _NativeEnds(_VersionedPlan):
+    """What the two fp16 plans with hand-written kernels share: the folded base plan, the kernel-layout weights (`_derive`, refreshed
+    into the SAME device tensors so that captured CUDA graphs stay valid) and the input contract: uint8 [B,96] canonical boards in,
+    float32 logits / value written in place."""
 
     precision = "fp16"
     dtype = torch.uint8
 
-    def __init__(self, net, max_batch, first_conv=None, owner=None):
-        """first_conv: "gather" (CUDA-core gather-add, k_first_conv; the default), "tc" (wgmma,
-        k_first_conv_tc) or "mma" (mma.sync with the one-hot operand built in registers: every warp re-reads the 36 KB weight
-        fragments from shared memory per 16-cell tile).  "tc" and "mma" are tested alternatives to the default."""
+    def __init__(self, net, max_batch, owner):
         import ctypes as C
         from ._lib import lib
         self._C, self._lib = C, lib()
-        self.first_conv = first_conv or os.environ.get("CCHESS_FIRST_CONV", "gather")
-        assert self.first_conv in ("gather", "tc", "mma")
-        base = InferencePlan(net, "fp16", owner=owner)
-        self.blocks, self.fused, self._base = base.blocks, base.fused, base
-        self.net, self.owner, self.version = net, owner, base.version
-        dev = base.w_in[0].device
+        self._base = InferencePlan(net, "fp16", owner=owner)
+        self.net, self.owner, self.version, self.max_batch = net, owner, self._base.version, max_batch
         for k, v in self._derive().items():
             setattr(self, k, v)
-        self.max_batch = max_batch
-        self.x1 = torch.empty((max_batch, 9, 10, 128), dtype=torch.float16, device=dev)
+        dev = self._base.w_in[0].device
         self.hp = torch.zeros((max_batch, 192), dtype=torch.float16, device=dev)
         self.hv = torch.zeros((max_batch, 96), dtype=torch.float32, device=dev)
-        # policy features in the tiled operand layout of the wgmma policy FC (rows beyond the batch stay zero)
-        self.hp_tiled = torch.zeros(((max_batch + 127) // 128, 24, 128, 8), dtype=torch.float16, device=dev)
-        self.heads = os.environ.get("CCHESS_HEADS", "tc")          # "tc": wgmma policy FC (batches >= 128); "mma": the mma.sync kernels
-
-    def _derive(self):
-        """Kernel-layout copies of the ends' weights, derived from the folded base plan."""
-        net, base = self.net, self._base
-        dev = base.w_in[0].device
-        with torch.no_grad():
-            w, b = base.w_in                                                    # folded conv_in: [128,14,3,3] fp16
-            w1 = w.float().permute(2, 3, 1, 0).reshape(9, 14, 128).to(torch.float16).contiguous()
-            b1 = b.float().contiguous()
-            # tensor-core variant: K = tap*16 + piece code (codes 0 / 15 are zero rows), canonical K-major no-swizzle tile
-            # [k-chunk (18)][8-channel group (16)][channel in group (8)][k in chunk (8)]
-            wpad = torch.zeros((9, 16, 128), dtype=torch.float16, device=dev)
-            wpad[:, 1:15, :] = w1
-            wpad[4, 15, :] = b1.to(torch.float16)            # bias rides in the GEMM: A has a constant 1 in (centre tap, slot 15)
-            wh, bh = base.w_head                                                 # [3,128,1,1]
-            wp = torch.zeros((2112, 192), dtype=torch.float16, device=dev)
-            wp[:NLABEL, :180] = net.p_fc.weight.detach().to(torch.float16)
-            bp = torch.zeros((2112,), dtype=torch.float32, device=dev)
-            bp[:NLABEL] = net.p_fc.bias.detach().float()
-            # policy FC weights as wgmma operand tiles: [17 label tiles][24 k-chunks][128 labels][8 features]
-            wp_pad = torch.zeros((2176, 192), dtype=torch.float16, device=dev)
-            wp_pad[:2112] = wp
-            bp_pad = torch.zeros((2176,), dtype=torch.float32, device=dev)
-            bp_pad[:2112] = bp
-            # m16n8k16 B-fragment order for k_first_conv_mma: [tap][n-tile][lane] -> ({W[2t][n], W[2t+1][n]}, {W[2t+8][n], W[2t+9][n]})
-            lanes = torch.arange(32, device=dev)
-            gg, tt = lanes // 4, lanes % 4
-            ncol = (torch.arange(16, device=dev)[:, None] * 8 + gg[None, :])                      # [16 tiles][32 lanes] -> channel
-            def krow(off):                                                                         # wpad[tap][2t+off][n] as [9,16,32]
-                return wpad[:, (2 * tt + off)[None, :].expand(16, 32), ncol]
-            frag = torch.stack([krow(0), krow(1), krow(8), krow(9)], dim=-1).contiguous()          # [9,16,32,4] fp16 = 2 words per lane
-            return dict(w1=w1, b1=b1, w1_umma=wpad.reshape(18, 8, 16, 8).permute(0, 2, 3, 1).contiguous(), w1_frag=frag,
-                        wp_tiled=wp_pad.reshape(17, 128, 24, 8).permute(0, 2, 1, 3).contiguous(), bp_pad=bp_pad,
-                        wh=wh.float().reshape(3, 128).contiguous(), bh=bh.float().contiguous(),
-                        w1t=net.v_fc1.weight.detach().float().t().contiguous(),        # [90,256]
-                        bv1=net.v_fc1.bias.detach().float().contiguous(),
-                        w2=net.v_fc2.weight.detach().float().reshape(256).contiguous(),
-                        b2t=net.v_fc2.bias.detach().float().reshape(1).contiguous(), wp=wp, bp=bp)
 
     def refresh(self):
-        """New weights into the SAME device tensors (captured CUDA graphs stay valid); see InferencePlan.refresh."""
+        """New weights into the SAME device tensors; see InferencePlan.refresh."""
         self._base.refresh()
         with torch.no_grad():
             for k, v in self._derive().items():
                 getattr(self, k).copy_(v)
         self.version = self._base.version
 
-    def refresh_if_stale(self):
-        if self.owner is not None and self.owner.weights_version != self.version:
-            self.refresh()
-            return True
-        return False
-
     def make_input(self, B):
-        return torch.zeros((B, 96), dtype=torch.uint8, device=self.x1.device)
+        return torch.zeros((B, 96), dtype=torch.uint8, device=self.hp.device)
+
+
+class NativePlan(_NativeEnds):
+    """fp16 inference plan whose ends are the hand-written kernels of csrc/cz_net.cu:
+         board bytes --cz_net_first_conv--> [B,90,128] --library cuDNN convs (residual tower)--> --cz_net_heads--> logits, value
+    Input is the engine's CZ_BOARD output (uint8 [B,96], the side-to-move-canonical board); the one-hot
+    [9,10,14] tensor is never built.  Outputs are written straight into the float32 buffers the engine reads.  Batches of 128 rows
+    or more take the wgmma policy FC (cz_net_heads_tc), smaller ones the mma.sync kernels (cz_net_heads)."""
+
+    first_conv = "gather"        # the first convolution is a gather-add of weight rows (k_first_conv)
+
+    def __init__(self, net, max_batch, owner=None):
+        super().__init__(net, max_batch, owner)
+        self.blocks, self.fused = self._base.blocks, self._base.fused
+        dev = self.hp.device
+        self.x1 = torch.empty((max_batch, 9, 10, 128), dtype=torch.float16, device=dev)
+        # policy features in the tiled operand layout of the wgmma policy FC (rows beyond the batch stay zero)
+        self.hp_tiled = torch.zeros(((max_batch + 127) // 128, 24, 128, 8), dtype=torch.float16, device=dev)
+
+    def _derive(self):
+        d = _ends_weights(self.net, self._base)
+        with torch.no_grad():
+            d["b1"] = self._base.w_in[1].float().contiguous()
+            # policy FC weights as wgmma operand tiles: [17 label tiles][24 k-chunks][128 labels][8 features]
+            wp_pad = torch.zeros((2176, 192), dtype=torch.float16, device=d["wp"].device)
+            wp_pad[:2112] = d["wp"]
+            d["bp_pad"] = torch.zeros((2176,), dtype=torch.float32, device=d["bp"].device)
+            d["bp_pad"][:2112] = d["bp"]
+            d["wp_tiled"] = wp_pad.reshape(17, 128, 24, 8).permute(0, 2, 1, 3).contiguous()
+        return d
 
     @torch.no_grad()
     def __call__(self, boards, logits_out, value_out):
         B = boards.shape[0]
         assert B <= self.max_batch and boards.dtype == torch.uint8 and logits_out.dtype == torch.float32
         st = self._C.c_void_p(torch.cuda.current_stream().cuda_stream)
-        if self.first_conv == "mma":
-            rc = self._lib.cz_net_first_conv_mma(boards.data_ptr(), B, self.w1_frag.data_ptr(), self.x1.data_ptr(), st)
-        elif self.first_conv == "tc":
-            rc = self._lib.cz_net_first_conv_tc(boards.data_ptr(), B, self.w1_umma.data_ptr(), self.b1.data_ptr(), self.x1.data_ptr(), st)
-        else:
-            rc = self._lib.cz_net_first_conv(boards.data_ptr(), B, self.w1.data_ptr(), self.b1.data_ptr(), self.x1.data_ptr(), st)
+        rc = self._lib.cz_net_first_conv(boards.data_ptr(), B, self.w1.data_ptr(), self.b1.data_ptr(), self.x1.data_ptr(), st)
         if rc:
-            raise RuntimeError("cz_net_first_conv (%s) failed (%d)" % (self.first_conv, rc))
+            raise RuntimeError("cz_net_first_conv failed (%d)" % rc)
         x = self.x1[:B].permute(0, 3, 1, 2)                                     # NCHW view of NHWC memory = channels_last
         for c1, c2 in self.blocks:
             y = self._base._conv_relu(x, c1, 1)
             x = self._base._conv_add_relu(y, c2, x)
         if not x.is_contiguous(memory_format=torch.channels_last):
             x = x.contiguous(memory_format=torch.channels_last)
-        if self.heads == "tc" and B >= 128:
+        if B >= 128:
             rc = self._lib.cz_net_heads_tc(x.data_ptr(), B, self.wh.data_ptr(), self.bh.data_ptr(), self.w1t.data_ptr(), self.bv1.data_ptr(),
                                            self.w2.data_ptr(), self.b2t.data_ptr(), self.wp_tiled.data_ptr(), self.bp_pad.data_ptr(),
                                            self.hp_tiled.data_ptr(), self.hv.data_ptr(), logits_out.data_ptr(), value_out.data_ptr(), st)
@@ -455,70 +449,31 @@ class NativePlan:
         return None
 
 
-class SmallTowerPlan:
+class SmallTowerPlan(_NativeEnds):
     """fp16 plan for a FEW positions (play mode, single-tree search; BASELINE config 5): the whole convolutional trunk runs in
-    ONE launch of csrc/cz_tower.cu (a thread-block cluster per position, activations resident in shared memory, weights streamed
-    by TMA, wgmma accumulating in registers), followed by the value MLP || policy FC kernels of csrc/cz_net.cu:
+    ONE launch of csrc/cz_tower.cu (a thread-block cluster of 4 CTAs per position, activations resident in shared memory, weights
+    streamed by TMA, wgmma accumulating in registers), followed by the value MLP || policy FC kernels of csrc/cz_net.cu:
         board bytes --cz_net_tower_small--> head features --cz_net_heads_fc--> logits, value            (3 kernels per evaluation)
-    Same input / output contract as NativePlan (uint8 [B,96] canonical boards in, float32 logits / value written in place)."""
+    Same input / output contract as NativePlan."""
 
-    precision = "fp16"
-    dtype = torch.uint8
     first_conv = "tower"
+    CL = 4                       # CTAs per cluster in csrc/cz_tower.cu: CTA r computes output channels [32 r, 32 r + 32)
 
-    def __init__(self, net, max_batch, cluster=None, owner=None):
-        import ctypes as C
-        from ._lib import lib
-        self._C, self._lib = C, lib()
-        self.cluster = int(cluster or os.environ.get("CCHESS_TOWER_CLUSTER", "4"))
-        assert self.cluster in (1, 2, 4, 8)
-        self._base = InferencePlan(net, "fp16", owner=owner)
+    def __init__(self, net, max_batch, owner=None):
+        super().__init__(net, max_batch, owner)
         self.fused = True
-        self.net, self.owner, self.version = net, owner, self._base.version
         self.n_conv = 2 * len(self._base.blocks)
-        for k, v in self._derive().items():
-            setattr(self, k, v)
-        dev = self._base.w_in[0].device
-        self.max_batch = max_batch
-        self.hp = torch.zeros((max_batch, 192), dtype=torch.float16, device=dev)
-        self.hv = torch.zeros((max_batch, 96), dtype=torch.float32, device=dev)
 
     def _derive(self):
-        net, base, CL = self.net, self._base, self.cluster
+        base, CL = self._base, self.CL
         NC = 128 // CL
-        dev = base.w_in[0].device
+        d = _ends_weights(self.net, base)
         with torch.no_grad():
-            w, b = base.w_in
-            w1 = w.float().permute(2, 3, 1, 0).reshape(9, 14, 128).to(torch.float16).contiguous()
             convs = [c for blk in base.blocks for c in blk]                       # (w [128,128,3,3] fp16, b [128]) in execution order
-            bias = torch.stack([b.float()] + [cb.float() for _, cb in convs]).contiguous()
+            d["bias"] = torch.stack([base.w_in[1].float()] + [cb.float() for _, cb in convs]).contiguous()
             # [conv][tap][rank][k-chunk 16][out channel NC][8 in channels]: the shared-memory image of one TMA stage, see cz_tower.cu
-            blob = torch.stack([cw.permute(2, 3, 0, 1).reshape(9, CL, NC, 16, 8).permute(0, 1, 3, 2, 4) for cw, _ in convs]).to(torch.float16).contiguous()
-            wh, bh = base.w_head
-            wp = torch.zeros((2112, 192), dtype=torch.float16, device=dev)
-            wp[:NLABEL, :180] = net.p_fc.weight.detach().to(torch.float16)
-            bp = torch.zeros((2112,), dtype=torch.float32, device=dev)
-            bp[:NLABEL] = net.p_fc.bias.detach().float()
-            return dict(w1=w1, bias=bias, blob=blob, wh=wh.float().reshape(3, 128).contiguous(), bh=bh.float().contiguous(),
-                        w1t=net.v_fc1.weight.detach().float().t().contiguous(), bv1=net.v_fc1.bias.detach().float().contiguous(),
-                        w2=net.v_fc2.weight.detach().float().reshape(256).contiguous(),
-                        b2t=net.v_fc2.bias.detach().float().reshape(1).contiguous(), wp=wp, bp=bp)
-
-    def refresh(self):
-        self._base.refresh()
-        with torch.no_grad():
-            for k, v in self._derive().items():
-                getattr(self, k).copy_(v)
-        self.version = self._base.version
-
-    def refresh_if_stale(self):
-        if self.owner is not None and self.owner.weights_version != self.version:
-            self.refresh()
-            return True
-        return False
-
-    def make_input(self, B):
-        return torch.zeros((B, 96), dtype=torch.uint8, device=self.hp.device)
+            d["blob"] = torch.stack([cw.permute(2, 3, 0, 1).reshape(9, CL, NC, 16, 8).permute(0, 1, 3, 2, 4) for cw, _ in convs]).to(torch.float16).contiguous()
+        return d
 
     @torch.no_grad()
     def __call__(self, boards, logits_out, value_out):
@@ -526,7 +481,7 @@ class SmallTowerPlan:
         assert B <= self.max_batch and boards.dtype == torch.uint8 and logits_out.dtype == torch.float32
         assert self.blob.numel() * 2 == self._lib.cz_net_tower_blob_bytes(self.n_conv)
         st = self._C.c_void_p(torch.cuda.current_stream().cuda_stream)
-        rc = self._lib.cz_net_tower_small(boards.data_ptr(), B, self.cluster, self.n_conv, self.w1.data_ptr(), self.blob.data_ptr(), self.bias.data_ptr(),
+        rc = self._lib.cz_net_tower_small(boards.data_ptr(), B, self.n_conv, self.w1.data_ptr(), self.blob.data_ptr(), self.bias.data_ptr(),
                                           self.wh.data_ptr(), self.bh.data_ptr(), self.hp.data_ptr(), self.hv.data_ptr(), st)
         if rc:
             raise RuntimeError("cz_net_tower_small failed (%d)" % rc)
@@ -624,14 +579,17 @@ class policy_value_network(object):
         return self._plan
 
     def native_plan(self, max_batch, first_conv=None):
-        """fp16 plan with the hand-written first-conv / head kernels (engine path); see NativePlan."""
+        """fp16 plan with the hand-written first-conv / head kernels (engine path); see NativePlan.  first_conv names the first-layer
+        kernel: None or "gather" (the gather-add, the only one there is)."""
+        if first_conv not in (None, "gather"):
+            raise ValueError("first_conv=%r: the 'tc' and 'mma' first-convolution variants were removed; only 'gather' remains" % (first_conv,))
         self.net.eval()
-        return NativePlan(self.net, max_batch, first_conv, owner=self)
+        return NativePlan(self.net, max_batch, owner=self)
 
-    def small_plan(self, max_batch, cluster=None):
+    def small_plan(self, max_batch):
         """fp16 plan for <= 16 positions per call: the whole trunk in one cluster kernel (csrc/cz_tower.cu); see SmallTowerPlan."""
         self.net.eval()
-        return SmallTowerPlan(self.net, max_batch, cluster, owner=self)
+        return SmallTowerPlan(self.net, max_batch, owner=self)
 
     @property
     def nn_dtype(self):

@@ -226,15 +226,6 @@ int cz_engine_tree_signature(cz_engine *e, void *stream, int game, int64_t *out,
  *     w2 [256], b2 [1] (device pointers, so that weights can be refreshed under a captured CUDA graph): value MLP; wp fp16 [2112][192] / bp f32 [2112]: policy FC zero-padded; hp_scratch fp16 [B][192],
  *     hv_scratch f32 [B][96]. */
 int cz_net_first_conv(const uint8_t *canon_boards, int B, const void *w1, const float *b1, void *out, void *stream);
-/* Same result on the Hopper tensor cores (wgmma): the one-hot im2col matrix is built in shared memory, the accumulators live in
- * registers.  w_umma: dev fp16, the weights in the canonical K-major no-swizzle layout [18 k-chunks][16 groups][8 channels][8 k]
- * with k = tap*16 + piece code (code 0 rows are zero; row (centre tap, code 15) holds the bias, every other code-15 row is
- * zero); 36 864 bytes.  b1 is ignored (kept for signature symmetry with cz_net_first_conv). */
-int cz_net_first_conv_tc(const uint8_t *canon_boards, int B, const void *w_umma, const float *b1, void *out, void *stream);
-/* Same result on mma.sync with the one-hot operand built in registers (alternative first layer; slower than the gather-add, see DESIGN.md).  w_frag: dev, the
- * weights of cz_net_first_conv_tc's K = tap*16 + piece-code convention (bias row included) in m16n8k16 B-fragment order
- * [9 k-steps][16 n-tiles][32 lanes][2 words]: word0 = {W[k0+2t][n], W[k0+2t+1][n]}, word1 = the same at k + 8, n = 8*tile + lane/4, t = lane%4. */
-int cz_net_first_conv_mma(const uint8_t *canon_boards, int B, const void *w_frag, void *out, void *stream);
 int cz_net_heads(const void *x, int B, const float *wh, const float *bh, const float *w1t, const float *b1, const float *w2, const float *b2,
                  const void *wp, const float *bp, void *hp_scratch, float *hv_scratch, float *logits, float *value, void *stream);
 
@@ -266,23 +257,22 @@ int cz_net_heads_fc(const void *hp, const float *hv, int B, const float *w1t, co
  * policy_value_network.py:45-74, 151-162 with batch norm folded: first conv3x3(14->128) from the canonical board bytes,
  * n_conv = 2*res_block_nums 3x3 convolutions (residual blocks), the two 1x1 head convolutions; output = the head features
  * hp fp16 [n_pos][192] / hv f32 [n_pos][96] that cz_net_heads_fc turns into logits and value.
- * One thread-block cluster of `cluster` (1, 2, 4, 8) CTAs per position: activations stay in shared memory (K-major no-swizzle layout,
+ * One thread-block cluster of 4 CTAs per position: activations stay in shared memory (K-major no-swizzle layout,
  * 3x3 taps = descriptor start offsets), weights stream from L2 by TMA, wgmma accumulates in registers, epilogues exchange
  * channel slices through distributed shared memory.  See csrc/cz_tower.cu.
  *   w1     dev fp16 [9][14][128]   (as cz_net_first_conv);  bias dev f32 [1 + n_conv][128];  wh f32 [3][128], bh f32 [3]
- *   wblob  dev fp16, cz_net_tower_blob_bytes(n_conv) bytes, arranged for THIS cluster size:
- *          [conv][tap 9][rank `cluster`][k-chunk 16][out channel 128/cluster][8 in channels]   (in channel = 8*chunk + i) */
+ *   wblob  dev fp16, cz_net_tower_blob_bytes(n_conv) bytes, arranged by the CTA that reads each slice:
+ *          [conv][tap 9][rank 4][k-chunk 16][out channel 32][8 in channels]   (out channel = 32*rank + row, in channel = 8*chunk + i) */
 int64_t cz_net_tower_blob_bytes(int n_conv);
-int cz_net_tower_small(const uint8_t *canon_boards, int n_pos, int cluster, int n_conv, const void *w1, const void *wblob, const float *bias,
+int cz_net_tower_small(const uint8_t *canon_boards, int n_pos, int n_conv, const void *w1, const void *wblob, const float *bias,
                        const float *wh, const float *bh, void *hp, float *hv, void *stream);
 
 /* ---- fp32-accurate inference on the tensor cores (net.py: SplitTf32Plan; policy_value_network.py:202-214 is fp32) ----
- * y dev f32 [n_pix][128] (NHWC activations) -> hi dev f32 [n_pix][128] = tf32(y) (round to the 10-bit mantissa) and
- * x2 dev fp16 [n_pix][256] = { (y - hi) * 2^11 | hi } (both exact in fp16).  A TF32 convolution of hi with hi(w) and an fp16
+ * The split of activations v dev f32 [n_pix][128] (NHWC): hi dev f32 [n_pix][128] = tf32(v) (round to the 10-bit mantissa) and
+ * x2 dev fp16 [n_pix][256] = { (v - hi) * 2^11 | hi } (both exact in fp16).  A TF32 convolution of hi with hi(w) and an fp16
  * convolution of x2 with { hi(w) | lo(w) * 2^11 } accumulate hi*hi and (lo*hi + hi*lo) * 2^11 in two separate f32 chains (the
- * tensor cores' accumulator truncates, measured -6.6e-9 relative per accumulated term: the full-size terms get the short chain). */
-int cz_net_split_tf32(const float *y, float *hi, void *x2, long long n_pix, void *stream);
-/* The f32 epilogue of such a convolution fused with the split for the next one, one streaming pass:
+ * tensor cores' accumulator truncates, measured -6.6e-9 relative per accumulated term: the full-size terms get the short chain).
+ * cz_net_epilogue_split is the f32 epilogue of such a convolution fused with the split for the next one, one streaming pass:
  *   v = ReLU(t + 2^-11 s + bias [+ skip]);   x = v (optional);   hi, x2 = split of v (optional, both or neither)
  * t dev f32 [n_pix][128] (hi*hi, raw); s dev fp16 [n_pix][128] or NULL (cross terms, raw, scaled by 2^11); bias dev f32 [128];
  * skip dev f32 [n_pix][128] or NULL (x may alias skip). */

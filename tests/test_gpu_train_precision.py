@@ -107,8 +107,8 @@ def test_precision_at_realistic_logit_scale(blocks):
 
 
 def test_tf32_split_kernel_matches_its_torch_statement_and_search_runs_in_tf32x3():
-    """csrc/cz_net.cu: k_split_tf32 == net.split_acts bit for bit (incl. negative values, zeros, denormal-sized residues), and a
-    whole search with precision="tf32x3" (engine planes -> SplitTf32Plan -> tree) gives the visit counts of the fp32 evaluator on
+    """csrc/cz_net.cu: k_epilogue_split == its torch statement (net.split_acts for the split) bit for bit (incl. zeros, 7 decades of
+    magnitude, denormal-sized residues), and a whole search with precision="tf32x3" (engine planes -> SplitTf32Plan -> tree) gives the visit counts of the fp32 evaluator on
     the same weights (both are ~1e-6 from the exact network, far below any PUCT decision margin of these positions)."""
     import ctypes as C
     from cchess_zero_b200._lib import lib
@@ -120,8 +120,11 @@ def test_tf32_split_kernel_matches_its_torch_statement_and_search_runs_in_tf32x3
         y[0, :4] = torch.tensor([0.0, -0.0, 1.0, -1.0], device="cuda")
         hi = torch.full((n_pix, 128), float("nan"), device="cuda")
         x2 = torch.full((n_pix, 256), float("nan"), device="cuda", dtype=torch.float16)
-        assert lib().cz_net_split_tf32(y.data_ptr(), hi.data_ptr(), x2.data_ptr(), n_pix, C.c_void_p(torch.cuda.current_stream().cuda_stream)) == 0
-        rh, r2 = split_acts(y.t().reshape(1, 128, n_pix, 1))
+        # the split alone: v = relu(|y| + 0) = |y| (no cross terms, no skip, no x output)
+        ya, zero = y.abs(), torch.zeros(128, device="cuda")
+        assert lib().cz_net_epilogue_split(ya.data_ptr(), None, zero.data_ptr(), None, None, hi.data_ptr(), x2.data_ptr(), n_pix,
+                                           C.c_void_p(torch.cuda.current_stream().cuda_stream)) == 0
+        rh, r2 = split_acts(ya.t().reshape(1, 128, n_pix, 1))
         assert torch.equal(hi.view(torch.int32), rh.reshape(128, n_pix).t().contiguous().view(torch.int32))
         assert torch.equal(x2.view(torch.int16), r2.reshape(256, n_pix).t().contiguous().view(torch.int16))
         assert int((hi.view(torch.int32) & 0x1FFF).abs().max()) == 0
@@ -297,10 +300,10 @@ def test_data_parallel_train_step_over_nccl(tmp_path):
     assert "NCCL_DP_OK 2" in r.stdout
 
 
-@pytest.mark.parametrize("blocks,cluster,npos", [(2, 1, 1), (2, 8, 3), (7, 1, 2), (7, 2, 1), (7, 4, 5), (7, 8, 16), (19, 8, 1)])
-def test_small_tower_cluster_kernel_matches_library_plan_and_fp64(blocks, cluster, npos):
+@pytest.mark.parametrize("blocks,npos", [(2, 1), (2, 3), (7, 1), (7, 2), (7, 5), (7, 16), (19, 1)])
+def test_small_tower_cluster_kernel_matches_library_plan_and_fp64(blocks, npos):
     """csrc/cz_tower.cu (whole trunk in one launch: TMA-streamed weights, wgmma with tap-shifted A descriptors, register epilogues
-    exchanging channel slices through distributed shared memory) against the cuDNN plan and an fp64 evaluation, for every cluster size."""
+    exchanging channel slices through distributed shared memory) against the cuDNN plan and an fp64 evaluation."""
     from cchess_zero_b200.net import NativePlan, PolicyValueNet, SmallTowerPlan
     torch.manual_seed(1)
     net = PolicyValueNet(blocks).eval()
@@ -317,13 +320,13 @@ def test_small_tower_cluster_kernel_matches_library_plan_and_fp64(blocks, cluste
     boards = torch.from_numpy(canon).cuda()
     lo = torch.zeros((npos, 2086), device="cuda"); vo = torch.zeros((npos,), device="cuda")
     lo2 = torch.zeros_like(lo); vo2 = torch.zeros_like(vo)
-    small = SmallTowerPlan(net, 16, cluster)
+    small = SmallTowerPlan(net, 16)
     small(boards, lo, vo)
     NativePlan(net, 16)(boards, lo2, vo2)
     torch.cuda.synchronize()
     e_small = max((lo.double().cpu() - rl).abs().max().item(), (vo.double().cpu() - rv.reshape(-1)).abs().max().item())
     e_lib = max((lo2.double().cpu() - rl).abs().max().item(), (vo2.double().cpu() - rv.reshape(-1)).abs().max().item())
-    print("max abs err vs fp64: cluster trunk (CL=%d) %.3g, library trunk %.3g" % (cluster, e_small, e_lib))
+    print("max abs err vs fp64: cluster trunk %.3g, library trunk %.3g" % (e_small, e_lib))
     assert e_small < max(1e-3, 1.25 * e_lib)              # as accurate as the library trunk (same fp16 arithmetic, fp32 accumulation)
     assert (lo - lo2).abs().max().item() < max(2e-3, 2 * e_lib) and (vo - vo2).abs().max().item() < max(2e-3, 2 * e_lib)
     small(boards, lo2, vo2)                               # run-to-run identical
@@ -333,8 +336,10 @@ def test_small_tower_cluster_kernel_matches_library_plan_and_fp64(blocks, cluste
 
 @pytest.mark.parametrize("B", [128, 203, 1024])
 def test_tcgen05_policy_fc_and_mma_head_conv_match_the_simt_heads(B):
-    """cz_net_heads_tc (mma.sync head conv writing wgmma-tiled features, wgmma policy FC, 8-position value MLP) against the round-1
-    kernels (cz_net_heads with CCHESS_HEAD_CONV=simt semantics) and against fp64, on a random trunk output."""
+    """cz_net_heads_tc (mma.sync head conv writing wgmma-tiled features, wgmma policy FC, 8-position value MLP), which NativePlan runs
+    for batches of 128 rows or more, against cz_net_heads (row-major features, mma.sync policy FC) on the same trunk output, and
+    against fp64."""
+    import ctypes as C
     from cchess_zero_b200.net import NativePlan, PolicyValueNet
     torch.manual_seed(2)
     net = PolicyValueNet(2).eval()
@@ -345,15 +350,17 @@ def test_tcgen05_policy_fc_and_mma_head_conv_match_the_simt_heads(B):
     net = net.cuda().to(memory_format=torch.channels_last)
     x, canon = _positions(B, seed=11)
     boards = torch.from_numpy(canon).cuda()
-    outs = {}
-    for mode in ("tc", "mma"):
-        plan = NativePlan(net, B)
-        plan.heads = mode
-        lo = torch.zeros((B, 2086), device="cuda"); vo = torch.zeros((B,), device="cuda")
-        plan(boards, lo, vo)
-        plan(boards, lo, vo)
-        torch.cuda.synchronize()
-        outs[mode] = (lo, vo)
+    plan = NativePlan(net, B)
+    lo = torch.zeros((B, 2086), device="cuda"); vo = torch.zeros((B,), device="cuda")
+    plan(boards, lo, vo)
+    plan(boards, lo, vo)
+    lo2 = torch.zeros_like(lo); vo2 = torch.zeros_like(vo)
+    trunk = plan._keep                                                      # the trunk output the wgmma heads just read
+    assert plan._lib.cz_net_heads(trunk.data_ptr(), B, plan.wh.data_ptr(), plan.bh.data_ptr(), plan.w1t.data_ptr(), plan.bv1.data_ptr(),
+                                  plan.w2.data_ptr(), plan.b2t.data_ptr(), plan.wp.data_ptr(), plan.bp.data_ptr(), plan.hp.data_ptr(),
+                                  plan.hv.data_ptr(), lo2.data_ptr(), vo2.data_ptr(), C.c_void_p(torch.cuda.current_stream().cuda_stream)) == 0
+    torch.cuda.synchronize()
+    outs = {"tc": (lo, vo), "mma": (lo2, vo2)}
     with torch.no_grad():
         rl, rv = net.double()(torch.from_numpy(x).double().cuda())
     d_l = (outs["tc"][0] - outs["mma"][0]).abs().max().item()

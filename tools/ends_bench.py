@@ -1,5 +1,5 @@
 """Device time of the hand-written network-end kernels at the bench batch (CUDA events, 300 back-to-back launches each, warm)."""
-import contextlib, io, json, os, sys
+import contextlib, io, json, sys
 sys.path.insert(0, '.')
 import ctypes as C
 import torch
@@ -46,9 +46,7 @@ def timed(fn, n=300):
 
 
 out = {}
-out["first_conv_gather_us"] = timed(lambda: lib.cz_net_first_conv(boards.data_ptr(), B, plan.w1.data_ptr(), plan.b1.data_ptr(), plan.x1.data_ptr(), st), )
-out["first_conv_mma_us"] = timed(lambda: lib.cz_net_first_conv_mma(boards.data_ptr(), B, plan.w1_frag.data_ptr(), plan.x1.data_ptr(), st))
-out["first_conv_tc_us"] = timed(lambda: lib.cz_net_first_conv_tc(boards.data_ptr(), B, plan.w1_umma.data_ptr(), plan.b1.data_ptr(), plan.x1.data_ptr(), st))
+out["first_conv_gather_us"] = timed(lambda: lib.cz_net_first_conv(boards.data_ptr(), B, plan.w1.data_ptr(), plan.b1.data_ptr(), plan.x1.data_ptr(), st))
 heads = lambda: lib.cz_net_heads(x.data_ptr(), B, plan.wh.data_ptr(), plan.bh.data_ptr(), plan.w1t.data_ptr(), plan.bv1.data_ptr(), plan.w2.data_ptr(),
                                  plan.b2t.data_ptr(), plan.wp.data_ptr(), plan.bp.data_ptr(), plan.hp.data_ptr(), plan.hv.data_ptr(), lo.data_ptr(), vo.data_ptr(), st)
 out["heads_all_us"] = timed(heads)
@@ -58,5 +56,4 @@ out["heads_tc_all_us"] = timed(lambda: lib.cz_net_heads_tc(x.data_ptr(), B, plan
                                                            plan.b2t.data_ptr(), plan.wp_tiled.data_ptr(), plan.bp_pad.data_ptr(), plan.hp_tiled.data_ptr(), plan.hv.data_ptr(),
                                                            lo.data_ptr(), vo.data_ptr(), st))
 out["head_conv_us"] = out["heads_all_us"] - out["heads_fc_only_us"]
-out["head_conv_variant"] = os.environ.get("CCHESS_HEAD_CONV", "mma")
 print(json.dumps(dict(batch=B, **out)))

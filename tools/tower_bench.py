@@ -1,5 +1,5 @@
 """Per-call device time (CUDA events, warm L2, 200 calls) of the network evaluation at small batch: the one-launch cluster trunk
-(csrc/cz_tower.cu, every cluster size) vs the library trunk (cuDNN convs + csrc/cz_net.cu ends), eager and inside a CUDA graph."""
+(csrc/cz_tower.cu) vs the library trunk (cuDNN convs + csrc/cz_net.cu ends), eager and inside a CUDA graph."""
 import contextlib, io, json, sys
 sys.path.insert(0, '.')
 import torch
@@ -13,9 +13,7 @@ for B in (1, 8, 16):
     boards = torch.zeros((B, 96), dtype=torch.uint8, device="cuda")
     boards[:, :90] = torch.randint(0, 15, (B, 90), dtype=torch.uint8, device="cuda") * (torch.rand((B, 90), device="cuda") < 0.3)
     lo = torch.zeros((B, 2086), device="cuda"); vo = torch.zeros((B,), device="cuda")
-    plans = {"library_trunk": pv.native_plan(B)}
-    for cl in (1, 2, 4, 8):
-        plans["cluster_trunk_CL%d" % cl] = pv.small_plan(B, cl)
+    plans = {"library_trunk": pv.native_plan(B), "cluster_trunk": pv.small_plan(B)}
     for name, plan in plans.items():
         for _ in range(5):
             plan(boards, lo, vo)

@@ -1,13 +1,12 @@
-"""One evaluation by the cluster trunk (for ncu): python tools/tower_probe.py <cluster> [blocks]"""
+"""One evaluation by the cluster trunk (for ncu): python tools/tower_probe.py [blocks]"""
 import contextlib, io, sys
 sys.path.insert(0, '.')
 import torch
 from cchess_zero_b200.net import policy_value_network
-cl = int(sys.argv[1]) if len(sys.argv) > 1 else 8
-blocks = int(sys.argv[2]) if len(sys.argv) > 2 else 7
+blocks = int(sys.argv[1]) if len(sys.argv) > 1 else 7
 with contextlib.redirect_stdout(io.StringIO()):
     pv = policy_value_network(res_block_nums=blocks)
-plan = pv.small_plan(1, cl)
+plan = pv.small_plan(1)
 boards = torch.zeros((1, 96), dtype=torch.uint8, device="cuda")
 lo = torch.zeros((1, 2086), device="cuda"); vo = torch.zeros((1,), device="cuda")
 for _ in range(30):

@@ -24,10 +24,7 @@ for it in range(300):
     t[0].record()
     e.wave(sp.nn_in, sp.logits, sp.value)
     t[1].record()
-    if plan.first_conv == 'tc':
-        lib.cz_net_first_conv_tc(sp.nn_in.data_ptr(), B, plan.w1_umma.data_ptr(), plan.b1.data_ptr(), plan.x1.data_ptr(), st)
-    else:
-        lib.cz_net_first_conv(sp.nn_in.data_ptr(), B, plan.w1.data_ptr(), plan.b1.data_ptr(), plan.x1.data_ptr(), st)
+    lib.cz_net_first_conv(sp.nn_in.data_ptr(), B, plan.w1.data_ptr(), plan.b1.data_ptr(), plan.x1.data_ptr(), st)
     t[2].record()
     x = plan.x1[:B].permute(0, 3, 1, 2)
     for c1, c2 in plan.blocks:
