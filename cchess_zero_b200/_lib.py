@@ -60,6 +60,10 @@ def _sig(L):
     L.cz_engine_status.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp]
     L.cz_engine_counters.argtypes = [vp, vp, vp]
     L.cz_engine_tree_signature.argtypes = [vp, vp, i32, vp, i64, vp]
+    L.cz_engine_snapshot_size.argtypes = [vp, vp, vp]
+    L.cz_engine_snapshot.argtypes = [vp, vp, vp, i64, vp]
+    L.cz_engine_restore.argtypes = [vp, vp, vp, i64]
+    L.cz_snapshot_check.argtypes = [vp, i64, i32, i32, i32, i64]
     L.cz_net_first_conv.argtypes = [vp, i32, vp, vp, vp, vp]
     L.cz_net_heads.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.cz_host_choose_moves.argtypes = [i32, vp, vp, vp, i32, vp, vp, vp, vp, i32]

@@ -1385,6 +1385,50 @@ __global__ void k_apply(uint8_t *boards, const uint16_t *moves, int n, uint8_t *
     b[src] = 0;
 }
 
+// ---- engine snapshots (cz_engine_snapshot / cz_engine_restore) ----------------------------------------------------------
+// Between plies a game's whole state is its header line, its root board, its five counters, its FIFO event-loop words (FIFO
+// engines) and words [0, H_ALLOC) of its current arena half (play_child compacts the live tree to offset 0 and expansions
+// bump-allocate after it).  Blob: a 48-byte head, int64 word offsets of the B game sections and the end (the head padded to
+// 16 bytes), then per game: hdr [16] | root board [24] | counters 5 x u64 [10] | pad [2] | fifo [FW] (FIFO engines) | arena [alloc].
+// Every section is a multiple of 4 words at a 16-byte aligned offset, so both directions copy with copy_block.
+#define SNAP_MAGIC 0x485350414E535A43ull   // "CZSNAPSH"
+#define SNAP_FORMAT 1u
+#define SNAP_HEAD_WORDS 12                 // magic | format, cz_version | zobrist checksum | B, K | narr, fixed words | reserved
+enum { S_HDR = 0, S_BOARD = 16, S_CNT = 40, S_FIFO = 52 };
+
+__device__ __forceinline__ unsigned long long *counter_array(const Dev &E, int k) {
+    return k == 0 ? E.cnt_expand : k == 1 ? E.cnt_playout : k == 2 ? E.cnt_L : k == 3 ? E.cnt_c : E.cnt_C;
+}
+
+// One warp per game: its sections -> blob + off[g] (offsets: the exclusive scan of the section sizes, in the blob's head).
+__global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) k_snapshot_pack(Dev E, uint32_t *__restrict__ blob) {
+    const int lane = threadIdx.x & 31, g = blockIdx.x * WARPS_PER_BLOCK + (threadIdx.x >> 5);
+    if (g >= E.B) return;
+    uint32_t *s = blob + reinterpret_cast<const long long *>(blob + SNAP_HEAD_WORDS)[g];
+    const uint32_t *h = E.hdr + (size_t)g * HW;
+    copy_block(s + S_HDR, h, HW, lane);
+    copy_block(s + S_BOARD, reinterpret_cast<const uint32_t *>(E.root_board + (size_t)g * 96), 24, lane);
+    if (lane < 5) reinterpret_cast<unsigned long long *>(s + S_CNT)[lane] = counter_array(E, lane)[g];
+    if (lane == 5) { s[S_CNT + 10] = 0u; s[S_CNT + 11] = 0u; }
+    if (E.fifo) copy_block(s + S_FIFO, E.fifo + (size_t)g * FW, FW, lane);
+    const uint32_t flags = h[H_FLAGS], alloc = h[H_ALLOC];
+    copy_block(s + S_FIFO + (E.fifo ? FW : 0), arena_half(E, g, (flags & F_CUR) ? 1 : 0), alloc, lane);
+}
+
+// The inverse, into the engine's own buffers (a validated blob; pending leaf-parallel slots are cleared: the game is at rest).
+__global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) k_snapshot_unpack(Dev E, const uint32_t *__restrict__ blob) {
+    const int lane = threadIdx.x & 31, g = blockIdx.x * WARPS_PER_BLOCK + (threadIdx.x >> 5);
+    if (g >= E.B) return;
+    const uint32_t *s = blob + reinterpret_cast<const long long *>(blob + SNAP_HEAD_WORDS)[g];
+    copy_block(E.hdr + (size_t)g * HW, s + S_HDR, HW, lane);
+    copy_block(reinterpret_cast<uint32_t *>(E.root_board + (size_t)g * 96), s + S_BOARD, 24, lane);
+    if (lane < 5) counter_array(E, lane)[g] = reinterpret_cast<const unsigned long long *>(s + S_CNT)[lane];
+    if (E.fifo) copy_block(E.fifo + (size_t)g * FW, s + S_FIFO, FW, lane);
+    if (E.pendK) for (int i = lane; i < E.K; i += 32) E.pendK[(size_t)g * E.K + i] = 0;
+    const uint32_t flags = s[S_HDR + H_FLAGS], alloc = s[S_HDR + H_ALLOC];
+    copy_block(arena_half(E, g, (flags & F_CUR) ? 1 : 0), s + S_FIFO + (E.fifo ? FW : 0), alloc, lane);
+}
+
 const int16_t *device_label_table(int device) {
     static const int16_t *tab[64] = {nullptr};
     if (device < 0 || device >= 64) return nullptr;
@@ -1398,19 +1442,33 @@ const int16_t *device_label_table(int device) {
 }
 
 // Zobrist keys: 16 piece codes x 96 squares of splitmix64 output (fixed seed), entry [0][95] = side to move.
+std::vector<unsigned long long> zobrist_keys() {
+    std::vector<unsigned long long> z(16 * 96);
+    unsigned long long x = 0x9E3779B97F4A7C15ull;
+    for (auto &v : z) {
+        x += 0x9E3779B97F4A7C15ull;
+        unsigned long long t = x;
+        t = (t ^ (t >> 30)) * 0xBF58476D1CE4E5B9ull;
+        t = (t ^ (t >> 27)) * 0x94D049BB133111EBull;
+        v = t ^ (t >> 31);
+    }
+    return z;
+}
+// FNV-1a 64 over the little-endian bytes of the key table: a snapshot records it, so root keys are never restored under other keys
+unsigned long long zobrist_checksum() {
+    static const unsigned long long sum = [] {
+        unsigned long long h = 0xCBF29CE484222325ull;
+        for (unsigned long long v : zobrist_keys())
+            for (int i = 0; i < 8; i++) { h ^= (v >> (8 * i)) & 0xFFu; h *= 0x100000001B3ull; }
+        return h;
+    }();
+    return sum;
+}
 const unsigned long long *device_zobrist_table(int device) {
     static const unsigned long long *tab[64] = {nullptr};
     if (device < 0 || device >= 64) return nullptr;
     if (!tab[device]) {
-        std::vector<unsigned long long> z(16 * 96);
-        unsigned long long x = 0x9E3779B97F4A7C15ull;
-        for (auto &v : z) {
-            x += 0x9E3779B97F4A7C15ull;
-            unsigned long long t = x;
-            t = (t ^ (t >> 30)) * 0xBF58476D1CE4E5B9ull;
-            t = (t ^ (t >> 27)) * 0x94D049BB133111EBull;
-            v = t ^ (t >> 31);
-        }
+        const std::vector<unsigned long long> z = zobrist_keys();
         unsigned long long *p = nullptr;
         if (cudaMalloc(&p, z.size() * 8) != cudaSuccess) return nullptr;
         if (cudaMemcpy(p, z.data(), z.size() * 8, cudaMemcpyHostToDevice) != cudaSuccess) return nullptr;
@@ -1436,6 +1494,8 @@ struct cz_engine {
     uint32_t *h_hdr = nullptr;
     uint8_t *d_mask = nullptr, *d_boards = nullptr, *d_sides = nullptr;
     int32_t *d_rr = nullptr;
+    uint32_t *d_snap = nullptr;      // device staging of snapshot blobs, grown on demand
+    size_t snap_cap = 0;
 };
 
 extern "C" {
@@ -1727,6 +1787,7 @@ int cz_engine_destroy(cz_engine *e) {
     cudaSetDevice(e->device);
     cudaDeviceSynchronize();
     for (void *p : e->allocs) cudaFree(p);
+    cudaFree(e->d_snap);
     cudaFreeHost(e->h_n); cudaFreeHost(e->h_visits); cudaFreeHost(e->h_choice); cudaFreeHost(e->h_moves);
     cudaFreeHost(e->h_f); cudaFreeHost(e->h_status); cudaFreeHost(e->h_i32); cudaFreeHost(e->h_hdr);
     delete e;
@@ -2071,6 +2132,185 @@ int cz_engine_tree_signature(cz_engine *e, void *stream, int game, int64_t *out,
         if (nch > 0) stack.push_back({child, nch, 0});
     }
     *n = k;
+    return CZ_OK;
+}
+
+// ---- snapshots of games at rest --------------------------------------------------------------------------------------------
+extern "C++" {
+static int64_t snap_head_words(int64_t B) { return ((48 + 8 * (B + 1) + 15) & ~15ll) / 4; }
+static uint32_t snap_fixed_words(int narr) { return S_FIFO + (narr == 6 ? FW : 0); }
+// At rest: no leaf or root expansion pending and no playouts owed (cz_engine_unfinished's test).  Leaf-parallel slots are only
+// pending while playouts are owed (done + in flight <= target), so the header line decides for every engine kind.
+static bool header_at_rest(const uint32_t *h) {
+    const uint32_t f = h[H_FLAGS];
+    if (F_PEND(f)) return false;
+    return !(f & F_ACTIVE) || ((int)h[H_ROOTCNT] >= 0 && (int)h[H_DONE] >= (int)h[H_TARGET]);
+}
+static int snap_fail(long long g, const char *what) {
+    char buf[256];
+    if (g >= 0) snprintf(buf, sizeof buf, "cz_snapshot_check: game %lld: %s", g, what);
+    else snprintf(buf, sizeof buf, "cz_snapshot_check: %s", what);
+    return fail(CZ_EINVAL, buf);
+}
+// Every block reachable from the root of one game section (ar = its arena words [0, alloc)); nullptr or the failed check.  Blocks
+// reached must be disjoint (so play_child's compaction copies at most alloc words) and children lie above their parent (no cycle).
+static const char *check_tree(const uint32_t *ar, uint32_t alloc, uint32_t rbase, int rcnt, int narr) {
+    if (rcnt <= 0) return nullptr;
+    std::vector<uint8_t> used(alloc / 8 + 1, 0);        // 8-word granules covered by a reachable block
+    struct Fr { uint32_t base; int cnt; };
+    std::vector<Fr> st{{rbase, rcnt}};
+    while (!st.empty()) {
+        const Fr f = st.back();
+        st.pop_back();
+        if (f.cnt > CZ_MAXCHILD) return "block with more than 128 children";
+        const uint32_t cs = (uint32_t)((f.cnt + 7) & ~7), size = HDR + (uint32_t)narr * cs;
+        if ((f.base & 7u) || (uint64_t)f.base + size > alloc) return "block outside [0, alloc) or not 8-word aligned";
+        if (ar[f.base] != (uint32_t)f.cnt) return "block header count differs from the parent's META n_grandchildren";
+        for (uint32_t k = f.base / 8; k < (f.base + size) / 8; k++) {
+            if (used[k]) return "blocks overlap or a block is reached twice";
+            used[k] = 1;
+        }
+        const uint32_t *blk = ar + f.base + HDR;
+        for (int i = 0; i < f.cnt; i++) {
+            const uint32_t meta = blk[3 * cs + i], child = blk[4 * cs + i];
+            if ((meta & 127u) >= CZ_NSQ || ((meta >> 7) & 127u) >= CZ_NSQ || (meta & 0xC000u)) return "move square outside the board";
+            if (meta >> 24) return "META bits 24-31 set (a playout in flight or a claimed leaf)";
+            const int ngc = (int)((meta >> 16) & 0xFFu);
+            if (child == NONE) {
+                if (ngc) return "META n_grandchildren set on an unexpanded child";
+                continue;
+            }
+            if (ngc == 0) return "expanded child with META n_grandchildren 0";
+            if (child <= f.base) return "child pointer not above its parent's base";
+            st.push_back({child, ngc});
+        }
+    }
+    return nullptr;
+}
+// Section offsets of every game from the header lines (one device->host copy); refuses a game that is not at rest.
+static int snapshot_layout(cz_engine *e, void *stream, std::vector<int64_t> &off, const char *who) {
+    int rc = fetch_headers(e, stream);
+    if (rc) return rc;
+    const int B = e->d.B;
+    const uint32_t fixed = snap_fixed_words(e->d.narr);
+    off.assign((size_t)B + 1, snap_head_words(B));
+    for (int g = 0; g < B; g++) {
+        const uint32_t *h = e->h_hdr + (size_t)g * HW;
+        if (!header_at_rest(h)) {
+            char buf[160];
+            snprintf(buf, sizeof buf, "%s: game %d is not at rest (a search is in progress)", who, g);
+            return fail(CZ_EINVAL, buf);
+        }
+        off[g + 1] = off[g] + fixed + h[H_ALLOC];
+    }
+    return CZ_OK;
+}
+static int snapshot_staging(cz_engine *e, size_t bytes) {
+    if (bytes <= e->snap_cap) return CZ_OK;
+    cudaFree(e->d_snap);
+    e->d_snap = nullptr;
+    e->snap_cap = 0;
+    const size_t want = bytes + bytes / 4;
+    cudaError_t ce = cudaMalloc(&e->d_snap, want);
+    if (ce != cudaSuccess) { e->d_snap = nullptr; return fail(CZ_ENOMEM, "snapshot staging: cudaMalloc", ce); }
+    e->snap_cap = want;
+    return CZ_OK;
+}
+}  // extern "C++"
+
+int cz_snapshot_check(const void *in, int64_t bytes, int n_games, int leaves, int narr, int64_t arena_words) {
+    if (n_games <= 0 || leaves <= 0 || (narr != 5 && narr != 6) || arena_words <= 0) return snap_fail(-1, "bad engine arguments");
+    if (!in || bytes < 48) return snap_fail(-1, "truncated blob: shorter than its head");
+    if ((uintptr_t)in & 7) return snap_fail(-1, "blob not 8-byte aligned");
+    const uint64_t *head = (const uint64_t *)in;
+    if (head[0] != SNAP_MAGIC) return snap_fail(-1, "bad magic: not an engine snapshot");
+    if ((uint32_t)head[1] != SNAP_FORMAT) return snap_fail(-1, "unsupported format version");
+    if (head[2] != zobrist_checksum()) return snap_fail(-1, "Zobrist table checksum differs from this library's");
+    const int B = (int32_t)(uint32_t)head[3], K = (int32_t)(uint32_t)(head[3] >> 32), na = (int32_t)(uint32_t)head[4];
+    const uint32_t fixed = (uint32_t)(head[4] >> 32);
+    if (B != n_games) return snap_fail(-1, "n_games differs from the engine's");
+    if (K != leaves) return snap_fail(-1, "leaves per game (K) differs from the engine's");
+    if (na != narr) return snap_fail(-1, "arrays per node block (narr) differ from the engine's");
+    if (fixed != snap_fixed_words(narr)) return snap_fail(-1, "section head size differs from the format's");
+    const int64_t hw = snap_head_words(B);
+    if (bytes < hw * 4) return snap_fail(-1, "truncated blob: shorter than its offset table");
+    const int64_t *off = (const int64_t *)(head + 6);
+    if (off[0] != hw) return snap_fail(-1, "first section does not follow the offset table");
+    for (int g = 0; g < B; g++)
+        if (off[g + 1] < off[g] || off[g + 1] - off[g] < (int64_t)fixed) return snap_fail(g, "section offsets not monotone");
+    if ((bytes & 3) || off[B] != bytes / 4) return snap_fail(-1, "truncated or padded blob: the offsets do not sum to its size");
+    const uint32_t *w = (const uint32_t *)in;
+    for (int g = 0; g < B; g++) {
+        const uint32_t *s = w + off[g], *h = s + S_HDR;
+        const uint32_t alloc = h[H_ALLOC], f = h[H_FLAGS];
+        if (off[g + 1] - off[g] != (int64_t)fixed + alloc) return snap_fail(g, "section size differs from its head + alloc");
+        if ((int64_t)alloc > arena_words) return snap_fail(g, "alloc exceeds the engine's arena words");
+        if (alloc & 7u) return snap_fail(g, "alloc not a multiple of 8 words");
+        if (!header_at_rest(h)) return snap_fail(g, "not at rest: an expansion is pending or playouts are owed");
+        if (f & ~0xF1Fu) return snap_fail(g, "unknown flag bits");
+        const uint32_t term = F_TERM(f), win = (f >> 10) & 3u;
+        if (term == 3 || win == 3 || (term == 1) != (win != 0)) return snap_fail(g, "bad terminal / winner code");
+        const int rcnt = (int)h[H_ROOTCNT];
+        if (rcnt < -1 || rcnt > CZ_MAXCHILD) return snap_fail(g, "root child count outside {-1, 0..128}");
+        const uint8_t *b = (const uint8_t *)(s + S_BOARD);
+        for (int i = 0; i < 96; i++)
+            if (b[i] > (i < CZ_NSQ ? 14 : 0)) return snap_fail(g, "root board piece code outside 0..14 (or padding not zero)");
+        if (narr == 6 && (s[S_FIFO + FI_ITER] || s[S_FIFO + FI_NCUR] || s[S_FIFO + FI_NQ]))
+            return snap_fail(g, "FIFO event loop not at rest");
+        const char *why = check_tree(s + fixed, alloc, h[H_ROOTBASE], rcnt, narr);
+        if (why) return snap_fail(g, why);
+    }
+    return CZ_OK;
+}
+
+int cz_engine_snapshot_size(cz_engine *e, void *stream, int64_t *bytes) {
+    if (!e || !bytes) return fail(CZ_EINVAL, "cz_engine_snapshot_size: null");
+    std::vector<int64_t> off;
+    int rc = snapshot_layout(e, stream, off, "cz_engine_snapshot_size");
+    if (rc) return rc;
+    *bytes = off.back() * 4;
+    return CZ_OK;
+}
+
+int cz_engine_snapshot(cz_engine *e, void *stream, void *out, int64_t cap, int64_t *bytes) {
+    if (!e || !out || !bytes) return fail(CZ_EINVAL, "cz_engine_snapshot: null");
+    std::vector<int64_t> off;
+    int rc = snapshot_layout(e, stream, off, "cz_engine_snapshot");
+    if (rc) return rc;
+    const int B = e->d.B;
+    const int64_t hw = snap_head_words(B), total = off.back() * 4;
+    *bytes = total;
+    if (cap < total) return fail(CZ_EINVAL, "cz_engine_snapshot: cap is smaller than the snapshot (see cz_engine_snapshot_size)");
+    std::vector<uint64_t> head((size_t)hw / 2, 0ull);
+    head[0] = SNAP_MAGIC;
+    head[1] = SNAP_FORMAT | ((uint64_t)(uint32_t)cz_version() << 32);
+    head[2] = zobrist_checksum();
+    head[3] = (uint32_t)B | ((uint64_t)(uint32_t)e->d.K << 32);
+    head[4] = (uint32_t)e->d.narr | ((uint64_t)snap_fixed_words(e->d.narr) << 32);
+    memcpy(head.data() + 6, off.data(), off.size() * 8);
+    rc = snapshot_staging(e, (size_t)total);
+    if (rc) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    CUDA_TRY(cudaMemcpyAsync(e->d_snap, head.data(), (size_t)hw * 4, cudaMemcpyHostToDevice, st));
+    k_snapshot_pack<<<nblk(B, WARPS_PER_BLOCK), 32 * WARPS_PER_BLOCK, 0, st>>>(e->d, e->d_snap);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaMemcpyAsync(out, e->d_snap, (size_t)total, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return CZ_OK;
+}
+
+int cz_engine_restore(cz_engine *e, void *stream, const void *in, int64_t bytes) {
+    if (!e) return fail(CZ_EINVAL, "cz_engine_restore: null engine");
+    int rc = cz_snapshot_check(in, bytes, e->d.B, e->d.K, e->d.narr, e->d.A);   // nothing on the device is written before this
+    if (rc) return rc;
+    CUDA_TRY(cudaSetDevice(e->device));
+    rc = snapshot_staging(e, (size_t)bytes);
+    if (rc) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    CUDA_TRY(cudaMemcpyAsync(e->d_snap, in, (size_t)bytes, cudaMemcpyHostToDevice, st));
+    k_snapshot_unpack<<<nblk(e->d.B, WARPS_PER_BLOCK), 32 * WARPS_PER_BLOCK, 0, st>>>(e->d, e->d_snap);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaStreamSynchronize(st));
     return CZ_OK;
 }
 

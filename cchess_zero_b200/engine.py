@@ -201,6 +201,27 @@ class Engine:
             return self.tree_signature(game, int(n.value))
         return out[: n.value].copy()
 
+    # ---- snapshots of games at rest (cz_engine_snapshot / cz_engine_restore) ----------------
+    def snapshot(self):
+        """Every game's state as one self-describing uint8 blob; EngineError while a search is in progress."""
+        n = C.c_int64(0)
+        check(lib().cz_engine_snapshot_size(self.h, _stream(), C.byref(n)), "cz_engine_snapshot_size")
+        out = np.empty(n.value, dtype=np.uint8)
+        self.launches += 1
+        check(lib().cz_engine_snapshot(self.h, _stream(), _hp(out), out.nbytes, C.byref(n)), "cz_engine_snapshot")
+        return out
+
+    def restore(self, blob):
+        """Write a snapshot back in place (captured graphs stay valid).  The blob is validated first: a corrupt one, or one from an
+        engine of another shape, raises EngineError and leaves the engine untouched."""
+        b = np.ascontiguousarray(blob, dtype=np.uint8)
+        if b.ndim != 1:
+            raise ValueError("a snapshot is a 1-d uint8 array")
+        if b.ctypes.data % 8:                      # the validator reads the blob as 64-bit words
+            b = b.copy()
+        self.launches += 1
+        check(lib().cz_engine_restore(self.h, _stream(), _hp(b), b.nbytes), "cz_engine_restore")
+
     # ---- a whole search: MCTS_tree.main for every selected game ---------------------------
     def search(self, forward_dev, playouts, nn_in, logits, value, mask=None, check_every=1):
         """forward_dev(nn_in) must fill `logits` [B,2086] f32 and `value` [B] (or [B,1]) f32 in place

@@ -17,7 +17,7 @@ import numpy as np
 import torch
 
 from . import rules
-from ._lib import MAXCHILD, MT_WORDS, NLABEL, EngineError
+from ._lib import MAXCHILD, MT_WORDS, NLABEL, NSQ, EngineError
 from .engine import Engine
 
 
@@ -590,6 +590,77 @@ class SelfPlay:
         """Hand over (and forget) the games finished so far: keeps memory flat in long self-play runs."""
         out, self.finished = self.finished, []
         return out
+
+    # -- games in flight: save and restore between plies ------------------------------------------------
+    _LOG = (("boards", (NSQ,), np.uint8), ("n", (), np.int32), ("moves", (MAXCHILD,), np.uint16), ("visits", (MAXCHILD,), np.int32),
+            ("choice", (), np.int32))
+
+    def save_games(self, path):
+        """Every game in flight into one np.savez file (written to a temporary file, then renamed): the engine's trees and game state
+        (Engine.snapshot) and the host state -- boards, sides, live, the per-slot MT19937 states, plies, temperature and each slot's
+        unfinished record (its players and log span).  load_games continues exactly where this left off.  The finished games must
+        have been handed over with pop_finished first."""
+        if self.lanes is not None:
+            raise ValueError("save_games: the two-lane pipeline cannot be saved")
+        if self.finished:
+            raise ValueError("save_games: %d finished games were not drained with pop_finished()" % len(self.finished))
+        from .train import _savez
+        blob = self.engine.snapshot()
+        rows = [(lg, g) for g in range(self.B) for lg in self._span[g]]
+        log = {"log_" + k: np.asarray([lg[k][g] for lg, g in rows], dtype=dt).reshape((len(rows),) + shp) for k, shp, dt in self._LOG}
+        players = [self.records[g].players for g in range(self.B)]
+        _savez(path, engine=blob, boards=self.boards, sides=self.sides, live=self.live, mt=self._mt, plies=np.int64(self.plies),
+               temperature=np.asarray(self.temperature, dtype=np.float64), span_len=np.asarray([len(s) for s in self._span], dtype=np.int64),
+               players_len=np.asarray([len(p) for p in players], dtype=np.int64),
+               players=np.asarray([p for ps in players for p in ps], dtype=np.uint8), **log)
+
+    def load_games(self, path):
+        """Restore what save_games wrote into this SelfPlay (same number of games and engine kind; the engine is restored in place, so
+        a captured graph stays valid).  The file is read without pickle and checked; ValueError / EngineError leave everything as it
+        was."""
+        if self.lanes is not None:
+            raise ValueError("load_games: the two-lane pipeline cannot be restored")
+        with np.load(path, allow_pickle=False) as d:
+            a = {k: d[k] for k in d.files}
+        B = self.B
+        want = dict(engine=(None, np.uint8), boards=((B, NSQ), np.uint8), sides=((B,), np.uint8), live=((B,), np.bool_),
+                    mt=((B, MT_WORDS), np.uint32), plies=((), np.int64), span_len=((B,), np.int64), players_len=((B,), np.int64),
+                    players=(None, np.uint8), temperature=(None, np.float64))
+        rows = int(a["span_len"].sum()) if "span_len" in a else -1
+        for k, shp, dt in self._LOG:
+            want["log_" + k] = ((rows,) + shp, dt)
+        for k, (shp, dt) in want.items():
+            if k not in a or a[k].dtype != dt or (shp is not None and a[k].shape != shp):
+                raise ValueError("games file: '%s' missing or not %s %s" % (k, np.dtype(dt).name, shp))
+        if a["engine"].ndim != 1 or a["players"].ndim != 1 or a["temperature"].shape not in ((), (B,)):
+            raise ValueError("games file: bad engine / players / temperature shape")
+        if a["span_len"].min() < 0 or a["players_len"].min() < 0 or int(a["players_len"].sum()) != len(a["players"]):
+            raise ValueError("games file: bad span or player counts")
+        if a["boards"].max() > 14 or a["sides"].max() > 1 or (len(a["players"]) and a["players"].max() > 1) or a["plies"] < 0:
+            raise ValueError("games file: piece code, side or ply count out of range")
+        n = a["log_n"]
+        if len(n) and (n.min() < 0 or n.max() > MAXCHILD or (a["log_choice"] < 0).any() or (a["log_choice"] >= n).any()):
+            raise ValueError("games file: logged move count or choice out of range")
+        self.engine.restore(a["engine"])                     # validated as a whole before anything on the device is written
+        spans = a["span_len"]
+        L = int(spans.max()) if B else 0
+        entries = [{k: np.zeros((B,) + shp, dtype=dt) for k, shp, dt in self._LOG} for _ in range(L)]
+        r = 0
+        for g in range(B):                                   # a slot's span is the last span_len[g] plies: align them at the end
+            for j in range(L - int(spans[g]), L):
+                for k, _, _ in self._LOG:
+                    entries[j][k][g] = a["log_" + k][r]
+                r += 1
+        t = a["temperature"]
+        self.temperature = float(t) if t.ndim == 0 else t.copy()
+        self._span = [entries[L - int(spans[g]):] for g in range(B)]
+        self.records = [GameRecord(g, None, self.temperature) for g in range(B)]
+        ends = np.cumsum(a["players_len"])
+        for g in range(B):
+            self.records[g].players = [int(p) for p in a["players"][ends[g] - a["players_len"][g]:ends[g]]]
+        self.boards, self.sides, self.live = a["boards"].copy(), a["sides"].copy(), a["live"].copy()
+        self._mt[:] = a["mt"]
+        self.plies = int(a["plies"])
 
     def play_games(self, max_plies=100000):
         """Every slot plays ONE game to the end (auto_reset must be False)."""

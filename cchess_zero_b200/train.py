@@ -279,8 +279,10 @@ class Trainer:
     reference does no augmentation).
 
     save(dir) / load(dir) keep everything a run needs to continue: the network(s) with their optimizer state, the replay buffer,
-    the sampler's random state, every game slot's MT19937 state, lr_multiplier and the counters.  Games in flight are not saved:
-    a resumed run starts fresh games in every slot (drawing from the restored per-slot streams)."""
+    the sampler's random state, every game slot's MT19937 state, lr_multiplier, the counters and the games in flight
+    (SelfPlay.save_games: the engine's trees and each slot's unfinished record), so a resumed run plays on exactly as the
+    uninterrupted one.  A directory saved without games.npz resumes with fresh games in every slot (drawing from the restored
+    per-slot streams)."""
 
     def __init__(self, network, n_games, playouts, search_threads=1, batch_size=512, buffer_size=10000, epochs=5, kl_targ=0.025,
                  learning_rate=1e-3, updates_per_game=1, mirror=False, eval_every=0, eval_games=10, eval_playouts=None,
@@ -433,9 +435,10 @@ class Trainer:
                lr_multiplier=self.lr_multiplier, next_gate=self.next_gate,
                counters=np.asarray([self.games, self.positions, self.updates, self.train_steps, self.promotions, self.gates, self.plies],
                                    dtype=np.int64))
+        self.sp.save_games(os.path.join(directory, "games.npz"))
 
     def load(self, directory):
-        """Restore what save() wrote; the games in flight are replaced by fresh games."""
+        """Restore what save() wrote, the games in flight included; without games.npz every slot starts a fresh game."""
         with np.load(os.path.join(directory, "trainer.npz"), allow_pickle=False) as d:
             if d["mt"].shape != self.sp._mt.shape:
                 raise ValueError("saved run has %d game slots, this Trainer %d" % (d["mt"].shape[0], self.n_games))
@@ -449,7 +452,11 @@ class Trainer:
         if self.best is not None:
             _restore_network(self.best, os.path.join(directory, "best"))
         self.buffer.load(os.path.join(directory, "replay.npz"))
-        self._restart_games(mt)
+        games = os.path.join(directory, "games.npz")
+        if os.path.isfile(games):
+            self.sp.load_games(games)
+        else:
+            self._restart_games(mt)
 
     def _restart_games(self, mt):
         """Every slot starts a fresh game from the start position, drawing its moves from the stream mt[slot]."""

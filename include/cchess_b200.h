@@ -217,6 +217,33 @@ int cz_engine_counters(cz_engine *e, void *stream, int64_t *out /* [9] */);
  * (label index, N, W bits, P bits, Q bits, n_children), children in order. Returns record count via *n. */
 int cz_engine_tree_signature(cz_engine *e, void *stream, int game, int64_t *out, int64_t cap, int64_t *n);
 
+/* ---- snapshots of games at rest (save / restore a self-play run between plies) ----
+ * A game is AT REST when no leaf or root expansion is pending and no playouts are owed (every game after cz_engine_unfinished
+ * returned 0, after cz_engine_play, after a reset).  Its whole state is then its 16-word header line, its root board, its five
+ * counters, its FIFO event-loop words (cz_engine_create_fifo engines) and words [0, alloc) of its current arena half (the live tree:
+ * cz_engine_play compacts it to offset 0).  Blob layout (little-endian, 4-byte words):
+ *   head  u64 [6]: magic 0x485350414E535A43 ("CZSNAPSH") | format 1 (low 32 bits), cz_version() (high) | FNV-1a 64 checksum of the
+ *                  Zobrist key table | n_games (low), leaves K (high) | narr = arrays per node block, 5 or 6 (low), F (high)
+ *   off   i64 [n_games + 1]: word offset of every game's section and of the end; head + off padded to a multiple of 16 bytes
+ *   per game: hdr [16] | root board [24] (96 bytes) | counters u64 [5] (expand, playout, L, c, C) | pad [2] | fifo [28] (narr 6
+ *             only) | arena [alloc]  -- F = 52 (narr 5) or 80 (narr 6) words precede the arena, alloc = hdr[7]
+ * cz_engine_snapshot_size: the blob's size in bytes (synchronises stream).  cz_engine_snapshot: writes it to out (host, cap bytes;
+ * *bytes = its size), one pack kernel and one device->host copy.  Both return CZ_EINVAL when a game is not at rest, snapshot also
+ * when cap is too small.  cz_engine_restore: validates the whole blob first (cz_snapshot_check against this engine) and returns
+ * CZ_EINVAL naming the game and the failed check with the engine untouched; otherwise one host->device copy and one unpack
+ * kernel write it IN PLACE into the engine's buffers (captured CUDA graphs stay valid) and every game is at rest.  The arena size
+ * may differ from the saving engine's as long as every alloc fits.  Board hashing on / off is not part of a snapshot. */
+int cz_engine_snapshot_size(cz_engine *e, void *stream, int64_t *bytes);
+int cz_engine_snapshot(cz_engine *e, void *stream, void *out, int64_t cap, int64_t *bytes);
+int cz_engine_restore(cz_engine *e, void *stream, const void *in /* host */, int64_t bytes);
+/* Host only: the validator restore runs, for an engine of n_games x leaves with narr arrays per block and arena_words per half.
+ * Checks magic, format, Zobrist checksum, n_games / leaves / narr; offsets monotone and summing to the blob size; per game: alloc
+ * <= arena_words and a multiple of 8, header at rest with valid flag / terminal / winner codes, root child count in {-1, 0..128},
+ * root board piece codes 0..14, FIFO loop at rest; every block reachable from the root lies in [0, alloc), 8-word aligned, with a
+ * header count equal to its parent's META n_grandchildren and <= 128, blocks disjoint, child pointers above their parent's base,
+ * move squares < 90, META bits 24-31 clear.  CZ_OK or CZ_EINVAL (cz_last_error names the game and the check). */
+int cz_snapshot_check(const void *in, int64_t bytes, int n_games, int leaves, int narr, int64_t arena_words);
+
 /* ---- network ends (policy_value_network.py:45-48 and 55-74), hand-written; the residual tower is library code ----
  * cz_net_first_conv: canonical boards (dev u8 [B][96], from cz_engine_wave with CZ_BOARD) ->
  *     ReLU(conv3x3(14->128) + bias) as fp16 NHWC [B][90][128].  w1: dev fp16 [9 taps][14 pieces][128], b1: dev f32 [128]
