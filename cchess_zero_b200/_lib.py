@@ -45,8 +45,6 @@ def _sig(L):
     L.cz_engine_wave.argtypes = [vp, vp, vp, i32, vp, vp]
     L.cz_engine_wave_compact.argtypes = [vp, vp, vp, vp, i32, vp, vp]
     L.cz_engine_live_rows.argtypes = [vp, vp, vp]
-    L.cz_engine_select.argtypes = [vp, vp, vp, i32]
-    L.cz_engine_expand_backup.argtypes = [vp, vp, vp, vp]
     L.cz_engine_enable_hashing.argtypes = [vp, i32]
     L.cz_engine_leaf_hashes.argtypes = [vp, vp]
     L.cz_engine_root_keys.argtypes = [vp, vp, vp]

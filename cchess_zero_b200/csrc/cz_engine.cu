@@ -364,11 +364,10 @@ __device__ __forceinline__ uint32_t select_child(const BlockRegs &R, int cnt, in
 #define HGET(f) __shfl_sync(CZ_FULL, h, (f))
 #define HSET(f, v) do { if (lane == (f)) h = (uint32_t)(v); } while (0)
 
-// One wave for one game (one warp).  DO_EXPAND: consume the previous evaluation; DO_SELECT: run playouts
-// until the next leaf.
+// One wave for one game (one warp): consume the previous evaluation, then run playouts until the next leaf.
 // Launch shape: one CTA per SM whenever the games fit (warps per CTA = ceil(B / #SMs), <= MAX_WPB), so that every SM carries
 // the same number of game-warps; shared memory is sized per launch (sizeof(WarpSmem) per warp).
-template <typename T, bool DO_EXPAND, bool DO_SELECT>
+template <typename T>
 __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave(Dev E, T *nn_in, const float *logits, const float *value) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     WarpSmem *smem = reinterpret_cast<WarpSmem *>(smem_raw);
@@ -381,12 +380,11 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave(Dev E, T *nn_in, const
     uint32_t h = lane < HW ? hp[lane] : 0u;
     uint32_t lbw = 0, rbw = 0;
     if (lane < 24) {
-        if (DO_EXPAND) lbw = reinterpret_cast<const uint32_t *>(E.leaf_board + (size_t)g * 96)[lane];
-        if (DO_SELECT) rbw = reinterpret_cast<const uint32_t *>(E.root_board + (size_t)g * 96)[lane];
+        lbw = reinterpret_cast<const uint32_t *>(E.leaf_board + (size_t)g * 96)[lane];
+        rbw = reinterpret_cast<const uint32_t *>(E.root_board + (size_t)g * 96)[lane];
     }
-    uint2 pth = make_uint2(0, 0);
-    float val = 0.f;
-    if (DO_EXPAND) { pth = E.path[(size_t)g * MAXD + lane]; val = value[g]; }
+    const uint2 pth = E.path[(size_t)g * MAXD + lane];
+    const float val = value[g];
     uint32_t flags = HGET(H_FLAGS);
     if (!(flags & F_ACTIVE)) return;
     uint32_t *ar = arena_half(E, g, (flags & F_CUR) ? 1 : 0);
@@ -401,7 +399,7 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave(Dev E, T *nn_in, const
     BlockRegs R;
     bool have_root = false;
 
-    if (DO_EXPAND && pend) {
+    if (pend) {
         const int depth = pend == 1 ? plen : 0;
         // ---- round trip 2: the W / N words of the path (back-up operands) fly under the move generation ----
         uint32_t bW = 0, bN = 0;
@@ -430,7 +428,7 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave(Dev E, T *nn_in, const
             return;
         }
         // ---- round trip 3 (root block of the next descent) is requested BEFORE the logit gather (round trip 4) ----
-        if (DO_SELECT && pend == 1 && done < target) { load_block<false>(ar, root_base, root_cnt, lane, R); have_root = true; }
+        if (pend == 1 && done < target) { load_block<false>(ar, root_base, root_cnt, lane, R); have_root = true; }
         if (ok) {
             expand_write(ar, S, logits + (size_t)g * CZ_NLABEL, n, base, lane);
             if (pend == 2) { root_base = base; root_cnt = n; }
@@ -455,7 +453,7 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave(Dev E, T *nn_in, const
     }
 
     uint32_t maxdep = HGET(H_MAXDEPTH);
-    if (DO_SELECT && !pend) {
+    if (!pend) {
         const int side0 = (flags & F_SIDE) ? 1 : 0, rr0 = (int)HGET(H_RR);
         unsigned long long rhash = 0;
         if (E.hash_on) rhash = (unsigned long long)HGET(H_HASHLO) | ((unsigned long long)HGET(H_HASHHI) << 32);
@@ -546,7 +544,7 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave(Dev E, T *nn_in, const
             if (lane == 0 && accL) { atomicAdd(E.cnt_L + g, accL); atomicAdd(E.cnt_c + g, accC); }
         }
     }
-    if (DO_SELECT && E.hash_on && pend == 0 && lane == 0) E.leaf_hash[g] = 0ull;    // no leaf of this game in the batch
+    if (E.hash_on && pend == 0 && lane == 0) E.leaf_hash[g] = 0ull;    // no leaf of this game in the batch
     // ---- the header line goes back with one coalesced store ----
     HSET(H_FLAGS, F_SETPEND(flags, pend));
     HSET(H_DONE, done);
@@ -1837,28 +1835,12 @@ int cz_engine_begin_search(cz_engine *e, void *stream, const uint8_t *mask, int 
     return CZ_OK;
 }
 
-extern "C++" {
-template <bool X, bool S>
-static int launch_wave(cz_engine *e, void *stream, void *nn_in, int dt, const float *logits, const float *value) {
+int cz_engine_wave(cz_engine *e, void *stream, void *nn_in, int nn_dtype, const float *logits, const float *value) {
+    if (!e || !nn_in || !logits || !value) return fail(CZ_EINVAL, "cz_engine_wave: null");
     dim3 gr(nblk(e->d.B, e->wpb)), bl(32 * e->wpb);
     const size_t sm = (size_t)e->wpb * sizeof(WarpSmem);
     cudaStream_t st = (cudaStream_t)stream;
-    if (dt == CZ_F32) k_wave<float, X, S><<<gr, bl, sm, st>>>(e->d, (float *)nn_in, logits, value);
-    else if (dt == CZ_BF16) k_wave<__nv_bfloat16, X, S><<<gr, bl, sm, st>>>(e->d, (__nv_bfloat16 *)nn_in, logits, value);
-    else if (dt == CZ_F16) k_wave<__half, X, S><<<gr, bl, sm, st>>>(e->d, (__half *)nn_in, logits, value);
-    else if (dt == CZ_BOARD) k_wave<uint8_t, X, S><<<gr, bl, sm, st>>>(e->d, (uint8_t *)nn_in, logits, value);
-    else return fail(CZ_EINVAL, "wave: nn_dtype");
-    CUDA_TRY(cudaGetLastError());
-    return CZ_OK;
-}
-}  // extern "C++"
-
-int cz_engine_wave(cz_engine *e, void *stream, void *nn_in, int nn_dtype, const float *logits, const float *value) {
-    if (!e || !nn_in || !logits || !value) return fail(CZ_EINVAL, "cz_engine_wave: null");
     if (e->d.fifo) {    // search_threads = K schedule of the reference (canonical FIFO form)
-        dim3 gr(nblk(e->d.B, e->wpb)), bl(32 * e->wpb);
-        const size_t sm = (size_t)e->wpb * sizeof(WarpSmem);
-        cudaStream_t st = (cudaStream_t)stream;
         if (nn_dtype == CZ_F32) k_wave_fifo<float><<<gr, bl, sm, st>>>(e->d, (float *)nn_in, logits, value);
         else if (nn_dtype == CZ_BF16) k_wave_fifo<__nv_bfloat16><<<gr, bl, sm, st>>>(e->d, (__nv_bfloat16 *)nn_in, logits, value);
         else if (nn_dtype == CZ_F16) k_wave_fifo<__half><<<gr, bl, sm, st>>>(e->d, (__half *)nn_in, logits, value);
@@ -1868,9 +1850,6 @@ int cz_engine_wave(cz_engine *e, void *stream, void *nn_in, int nn_dtype, const 
         return CZ_OK;
     }
     if (e->d.pendK) {   // leaf-parallel engine
-        dim3 gr(nblk(e->d.B, e->wpb)), bl(32 * e->wpb);
-        const size_t sm = (size_t)e->wpb * sizeof(WarpSmem);
-        cudaStream_t st = (cudaStream_t)stream;
         if (nn_dtype == CZ_F32) k_wave_multi<float><<<gr, bl, sm, st>>>(e->d, (float *)nn_in, logits, value);
         else if (nn_dtype == CZ_BF16) k_wave_multi<__nv_bfloat16><<<gr, bl, sm, st>>>(e->d, (__nv_bfloat16 *)nn_in, logits, value);
         else if (nn_dtype == CZ_F16) k_wave_multi<__half><<<gr, bl, sm, st>>>(e->d, (__half *)nn_in, logits, value);
@@ -1879,7 +1858,13 @@ int cz_engine_wave(cz_engine *e, void *stream, void *nn_in, int nn_dtype, const 
         CUDA_TRY(cudaGetLastError());
         return CZ_OK;
     }
-    return launch_wave<true, true>(e, stream, nn_in, nn_dtype, logits, value);
+    if (nn_dtype == CZ_F32) k_wave<float><<<gr, bl, sm, st>>>(e->d, (float *)nn_in, logits, value);
+    else if (nn_dtype == CZ_BF16) k_wave<__nv_bfloat16><<<gr, bl, sm, st>>>(e->d, (__nv_bfloat16 *)nn_in, logits, value);
+    else if (nn_dtype == CZ_F16) k_wave<__half><<<gr, bl, sm, st>>>(e->d, (__half *)nn_in, logits, value);
+    else if (nn_dtype == CZ_BOARD) k_wave<uint8_t><<<gr, bl, sm, st>>>(e->d, (uint8_t *)nn_in, logits, value);
+    else return fail(CZ_EINVAL, "wave: nn_dtype");
+    CUDA_TRY(cudaGetLastError());
+    return CZ_OK;
 }
 // search_threads = K engines: one wave with row compaction.  nn_stage [B*K rows] receives every slot's input row as cz_engine_wave
 // would write it; nn_dense [B*K rows] receives the rows that need an evaluation, densely, in (game, slot) order; logits / value are
@@ -1910,17 +1895,6 @@ int cz_engine_live_rows(cz_engine *e, void *stream, int32_t *out_rows) {
     CUDA_TRY(cudaStreamSynchronize((cudaStream_t)stream));
     *out_rows = e->h_i32[8];
     return CZ_OK;
-}
-
-int cz_engine_select(cz_engine *e, void *stream, void *nn_in, int nn_dtype) {
-    if (!e || !nn_in) return fail(CZ_EINVAL, "cz_engine_select: null");
-    if (e->d.pendK) return fail(CZ_EINVAL, "cz_engine_select: leaf-parallel engines only support cz_engine_wave");
-    return launch_wave<false, true>(e, stream, nn_in, nn_dtype, nullptr, nullptr);
-}
-int cz_engine_expand_backup(cz_engine *e, void *stream, const float *logits, const float *value) {
-    if (!e || !logits || !value) return fail(CZ_EINVAL, "cz_engine_expand_backup: null");
-    if (e->d.pendK) return fail(CZ_EINVAL, "cz_engine_expand_backup: leaf-parallel engines only support cz_engine_wave");
-    return launch_wave<true, false>(e, stream, (void *)logits, CZ_F32, logits, value);
 }
 
 int cz_engine_enable_hashing(cz_engine *e, int on) {

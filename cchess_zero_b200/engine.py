@@ -93,14 +93,6 @@ class Engine:
         check(lib().cz_engine_live_rows(self.h, _stream(), C.byref(out)), "cz_engine_live_rows")
         return out.value
 
-    def select(self, nn_in):
-        self.launches += 1
-        check(lib().cz_engine_select(self.h, _stream(), nn_in.data_ptr(), _DT[nn_in.dtype]), "cz_engine_select")
-
-    def expand_backup(self, logits, value):
-        self.launches += 1
-        check(lib().cz_engine_expand_backup(self.h, _stream(), logits.data_ptr(), value.data_ptr()), "cz_engine_expand_backup")
-
     # ---- board hashing (Zobrist keys of the pending leaves; never used by the search) -------
     def enable_hashing(self, on=True):
         check(lib().cz_engine_enable_hashing(self.h, 1 if on else 0), "cz_engine_enable_hashing")
@@ -223,19 +215,44 @@ class Engine:
         check(lib().cz_engine_restore(self.h, _stream(), _hp(b), b.nbytes), "cz_engine_restore")
 
     # ---- a whole search: MCTS_tree.main for every selected game ---------------------------
-    def search(self, forward_dev, playouts, nn_in, logits, value, mask=None, check_every=1):
+    def search(self, forward_dev, playouts, nn_in, logits, value, mask=None):
         """forward_dev(nn_in) must fill `logits` [B,2086] f32 and `value` [B] (or [B,1]) f32 in place
         (device tensors).  Runs waves until every selected game has finished `playouts` playouts."""
         self.begin_search(playouts, mask)
-        waves = 0
-        while True:
-            self.wave(nn_in, logits, value)
-            waves += 1
-            first = playouts // self.leaves
-            if waves > first and (waves - first) % check_every == 0 and self.unfinished() == 0:
-                break
-            forward_dev(nn_in)
-            if waves > 4 * playouts + 64:
-                self.raise_on_error()
-                raise EngineError("search did not converge after %d waves" % waves)
-        return waves
+        return run_waves(self, lambda: self.wave(nn_in, logits, value), playouts // self.leaves, playouts,
+                         evaluate=lambda: forward_dev(nn_in))
+
+
+def run_waves(engine, step, min_waves, pmax, evaluate=None, may_stop=None, per_step=1):
+    """The wave loop of every search (after begin_search).  step() runs `per_step` waves -- for a captured graph, together with their
+    evaluations.  The search ends once more than `min_waves` waves have run, may_stop() (if given) holds and engine.unfinished() is 0;
+    until then evaluate() (if given) runs the network on the leaves of the last step.  A search still running after 4 * pmax + 64
+    waves (pmax: the largest playout count) raises EngineError: for the engine's error flags if any are set (raise_on_error), else
+    for the missing convergence.  Returns the number of waves."""
+    waves = 0
+    while True:
+        step()
+        waves += per_step
+        if waves > min_waves and (may_stop is None or may_stop()) and engine.unfinished() == 0:
+            return waves
+        if evaluate is not None:
+            evaluate()
+        if waves > 4 * pmax + 64:
+            engine.raise_on_error()
+            raise EngineError("search did not converge after %d waves" % waves)
+
+
+def capture_cuda_graph(body, warm, warmup, pool=None):
+    """body() captured into a new CUDA graph (on a fresh stream; pool: a memory pool shared with other graphs), after `warmup` runs
+    of warm() on a side stream: the first launches load modules and let libraries pick algorithms, which a capture must not do."""
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s):
+        for _ in range(warmup):
+            warm()
+    torch.cuda.current_stream().wait_stream(s)
+    torch.cuda.synchronize()
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g, pool=pool, stream=torch.cuda.Stream()):
+        body()
+    return g

@@ -17,7 +17,7 @@ import torch
 
 from . import rules
 from ._lib import NLABEL
-from .engine import Engine
+from .engine import Engine, capture_cuda_graph, run_waves
 
 
 class leaf_node(object):
@@ -162,34 +162,23 @@ class MCTS_tree(object):
         self._cache = None
 
     def _search_graph(self, playouts):
+        e = self.engine
         if self._graph is None:
-            s = torch.cuda.Stream()
-            s.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(s):
-                for _ in range(3):
-                    self._plan(self._nn_in, self._logits, self._value)
-            torch.cuda.current_stream().wait_stream(s)
-            torch.cuda.synchronize()
             # one playout at a time: several (wave -> evaluation) pairs per graph, so that the gap between two graph launches is paid
             # once per REPS playouts (a wave of a completed search does nothing: at most REPS - 1 idle evaluations per move)
             self._reps = int(os.environ.get("CCHESS_WAVES_PER_GRAPH", "8")) if self.K == 1 else 1
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
+
+            def body():
                 for _ in range(self._reps):
-                    self.engine.wave(self._nn_in, self._logits, self._value)
+                    e.wave(self._nn_in, self._logits, self._value)
                     self._plan(self._nn_in, self._logits, self._value)
-            self._graph = g
-        self.engine.begin_search(playouts)
-        waves = 0
-        while True:
+            self._graph = capture_cuda_graph(body, lambda: self._plan(self._nn_in, self._logits, self._value), 3)
+        e.begin_search(playouts)
+
+        def step():
             self._graph.replay()
-            self.engine.launches += self._reps
-            waves += self._reps
-            if waves > playouts // self.K and self.engine.unfinished() == 0:      # K leaves per wave: fewer waves needed
-                break
-            if waves > 4 * playouts + 64:
-                self.engine.raise_on_error()
-                raise RuntimeError("search did not converge")
+            e.launches += self._reps
+        run_waves(e, step, playouts // self.K, playouts, per_step=self._reps)      # K leaves per wave: fewer waves needed
 
     def generate_inputs(self, in_state, current_player):  # main.py:531-533
         return rules.encode_batch(rules.state_to_board(in_state)[None], [rules.side_of(current_player)])[0]

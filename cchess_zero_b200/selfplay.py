@@ -18,7 +18,7 @@ import torch
 
 from . import rules
 from ._lib import MAXCHILD, MT_WORDS, NLABEL, NSQ, EngineError
-from .engine import Engine
+from .engine import Engine, capture_cuda_graph, run_waves
 
 
 def _flip_board(b):
@@ -197,77 +197,6 @@ class GameRecord:
         return zip(self.states, self.dense_pi(), self.z)
 
 
-class _Lane:
-    """One half-batch of a pipelined SelfPlay: its own engine, I/O buffers and evaluator scratch."""
-
-    def __init__(self, engine, lo, hi, nn_in, logits, value, forward):
-        self.engine, self.lo, self.hi = engine, lo, hi
-        self.nn_in, self.logits, self.value, self.forward = nn_in, logits, value, forward
-
-
-class _MultiEngine:
-    """Engine-shaped facade over the lanes' engines (games [lo, hi) of lane k live in engine k)."""
-
-    def __init__(self, lanes, B):
-        self.lanes, self.B = lanes, B
-        self.device = lanes[0].engine.device
-
-    @property
-    def launches(self):
-        return sum(l.engine.launches for l in self.lanes)
-
-    def _m(self, mask, l):
-        return None if mask is None else np.ascontiguousarray(mask[l.lo:l.hi], dtype=np.uint8)
-
-    def reset(self, mask=None, boards=None, sides=None, rr=None):
-        for l in self.lanes:
-            if mask is not None and not np.any(mask[l.lo:l.hi]):
-                continue
-            l.engine.reset(self._m(mask, l), None if boards is None else boards[l.lo:l.hi],
-                           None if sides is None else sides[l.lo:l.hi], None if rr is None else rr[l.lo:l.hi])
-
-    def begin_search(self, playouts, mask=None):
-        for l in self.lanes:
-            l.engine.begin_search(playouts, self._m(mask, l))
-
-    def unfinished(self):
-        return sum(l.engine.unfinished() for l in self.lanes)
-
-    def root_children(self, want_wpq=True):
-        parts = [l.engine.root_children(want_wpq) for l in self.lanes]
-        return {k: (np.concatenate([p[k] for p in parts]) if parts[0][k] is not None else None) for k in parts[0]}
-
-    def play(self, child_index, want_status=True):
-        parts = [l.engine.play(child_index[l.lo:l.hi], want_status) for l in self.lanes]
-        return {k: np.concatenate([p[k] for p in parts]) for k in parts[0]} if want_status else None
-
-    def status(self, boards=True):
-        parts = [l.engine.status(boards) for l in self.lanes]
-        return {k: (np.concatenate([p[k] for p in parts]) if parts[0][k] is not None else None) for k in parts[0]}
-
-    def counters(self):
-        cs = [l.engine.counters() for l in self.lanes]
-        out = {k: sum(c[k] for c in cs) for k in ("n_expand", "n_playout", "sum_L", "sum_c", "sum_C")}
-        out["error"] = 0
-        for c in cs:
-            out["error"] |= c["error"]
-        out["max_arena_words"] = max(c["max_arena_words"] for c in cs)
-        out["max_depth"] = max(c["max_depth"] for c in cs)
-        out["first_error_game"] = next((l.lo + c["first_error_game"] for l, c in zip(self.lanes, cs) if c["first_error_game"] >= 0), -1)
-        return out
-
-    def raise_on_error(self):
-        for l in self.lanes:
-            l.engine.raise_on_error()
-        return self.counters()
-
-    def tree_signature(self, game):
-        for l in self.lanes:
-            if l.lo <= game < l.hi:
-                return l.engine.tree_signature(game - l.lo)
-        raise IndexError(game)
-
-
 class SelfPlay:
     """n_games concurrent self-play games on one engine, advanced in lock-step plies by step().
 
@@ -279,56 +208,42 @@ class SelfPlay:
     def __init__(self, n_games, forward, playouts, seeds=None, exploration=True, temperature=1,
                  nn_dtype=torch.float32, arena_words=0, auto_reset=True, device=None, keep_records=True, plan=None,
                  plan_factory=None, lanes=1, engine=None, hashing=False, search_threads=1, compact=None):
-        """plan: an InferencePlan / NativePlan (defines the input buffer, writes logits/value in place).
-        plan_factory(n) + lanes=2: two half-batches, each with its own engine and plan; the search pipelines them so
-        that one half's tree kernel runs under the other half's network (see capture_graph)."""
+        """plan: an InferencePlan / NativePlan (defines the input buffer, writes logits/value in place); plan_factory(rows) builds
+        one when `plan` is not given.  lanes: 1 is the only value."""
+        if lanes != 1:
+            raise ValueError("SelfPlay: lanes must be 1")
         self.B = n_games
         # search_threads = K > 1: every game runs the reference's K-coroutine schedule (k_wave_fifo); the network batch has K rows per game
         self.K = max(1, int(search_threads))
         # ... of which only the rows that carry a leaf are evaluated (row compaction, cz_engine_wave_compact): default for K > 1
-        self.compact = (self.K > 1 and lanes == 1 and engine is None) if compact is None else bool(compact)
-        assert not self.compact or (self.K > 1 and lanes == 1), "row compaction belongs to the search_threads = K engine"
-        if lanes > 1:
-            assert plan_factory is not None and n_games % lanes == 0
-            per = n_games // lanes
-            self.lanes = []
-            for k in range(lanes):
-                eng = Engine(per, arena_words, device)
-                dev = torch.device("cuda", eng.device)
-                pl = plan_factory(per)
-                lg = torch.zeros((per, NLABEL), dtype=torch.float32, device=dev)
-                vl = torch.zeros((per,), dtype=torch.float32, device=dev)
-                ni = pl.make_input(per)
-                self.lanes.append(_Lane(eng, k * per, (k + 1) * per, ni, lg, vl, (lambda x, pl=pl, lg=lg, vl=vl: pl(x, lg, vl))))
-            self.engine = _MultiEngine(self.lanes, n_games)
-            self.nn_in, self.logits, self.value, forward = None, None, None, None
+        self.compact = (self.K > 1 and engine is None) if compact is None else bool(compact)
+        assert not self.compact or self.K > 1, "row compaction belongs to the search_threads = K engine"
+        # `engine`: an object with the Engine interface (tests drive the host loop with a CPU stand-in); the product
+        # always constructs the CUDA engine here
+        self.engine = engine if engine is not None else (Engine(n_games, arena_words, device, search_threads=self.K) if self.K > 1
+                                                         else Engine(n_games, arena_words, device))
+        if hashing:                              # Zobrist keys of the pending leaves (must be on before a graph is captured)
+            self.engine.enable_hashing(True)
+        dev = torch.device("cuda", self.engine.device) if engine is None else torch.device(getattr(engine, "torch_device", "cpu"))
+        rows = n_games * self.K
+        if plan is None and plan_factory is not None:
+            plan = plan_factory(rows)
+        self.logits = torch.zeros((rows, NLABEL), dtype=torch.float32, device=dev)
+        self.value = torch.zeros((rows,), dtype=torch.float32, device=dev)
+        if plan is not None:
+            self.nn_in = plan.make_input(rows)
+            forward = lambda x: plan(x, self.logits, self.value)  # noqa: E731
         else:
-            # `engine`: an object with the Engine interface (tests drive the host loop with a CPU stand-in); the product
-            # always constructs the CUDA engine here
-            self.engine = engine if engine is not None else (Engine(n_games, arena_words, device, search_threads=self.K) if self.K > 1
-                                                             else Engine(n_games, arena_words, device))
-            if hashing:                              # Zobrist keys of the pending leaves (must be on before a graph is captured)
-                self.engine.enable_hashing(True)
-            dev = torch.device("cuda", self.engine.device) if engine is None else torch.device(getattr(engine, "torch_device", "cpu"))
-            rows = n_games * self.K
-            if plan is None and plan_factory is not None:
-                plan = plan_factory(rows)
-            self.logits = torch.zeros((rows, NLABEL), dtype=torch.float32, device=dev)
-            self.value = torch.zeros((rows,), dtype=torch.float32, device=dev)
-            if plan is not None:
-                self.nn_in = plan.make_input(rows)
-                forward = lambda x: plan(x, self.logits, self.value)  # noqa: E731
-            else:
-                self.nn_in = torch.zeros((rows, 9, 10, 14), dtype=nn_dtype, device=dev)
-            if self.compact:                                   # the engine writes every slot's row here; the leaves go densely to nn_in
-                self.nn_stage = torch.zeros_like(self.nn_in)
-                self._bucket_graphs, self._use_graphs, self._pool = {}, False, None
-                self.rows_evaluated = 0
-                # batch sizes the network is run at: multiples of the game count (K sizes, one lazily captured CUDA graph each).  Finer
-                # buckets evaluate 3.5 % fewer rows but a search then meets dozens of sizes, and capturing their graphs costs more
-                # than it saves in anything but a very long run (measured: 2.32 -> 1.81 M exp/s over 6 plies with 256-row buckets)
-                self.bucket_rows = n_games
-            self.lanes = None
+            self.nn_in = torch.zeros((rows, 9, 10, 14), dtype=nn_dtype, device=dev)
+        if self.compact:                                   # the engine writes every slot's row here; the leaves go densely to nn_in
+            self.nn_stage = torch.zeros_like(self.nn_in)
+            self._bucket_graphs, self._use_graphs, self._pool = {}, False, None
+            self.rows_evaluated = 0
+            # batch sizes the network is run at: multiples of the game count (K sizes, one lazily captured CUDA graph each).  Finer
+            # buckets evaluate 3.5 % fewer rows but a search then meets dozens of sizes, and capturing their graphs costs more
+            # than it saves in anything but a very long run (measured: 2.32 -> 1.81 M exp/s over 6 plies with 256-row buckets)
+            self.bucket_rows = n_games
+        self.lanes = None                                  # one engine and one network batch (bench.py reads the attribute)
         self.plan = plan
         self.forward = forward
         self.playouts = np.broadcast_to(np.asarray(playouts, dtype=np.int64), (n_games,)).copy()
@@ -364,63 +279,6 @@ class SelfPlay:
             self.logits.copy_(lo.reshape(self.B * self.K, NLABEL))
             self.value.copy_(v.reshape(self.B * self.K))
 
-    def _capture_pipeline(self, warmup=3):
-        """Two-lane software pipeline in ONE CUDA graph:
-              stage 1:  network(A)  ||  k_wave(B)        stage 2:  network(B)  ||  k_wave(A)
-        k_wave is a latency-bound kernel (one warp per game, ~17 % issue utilisation), so it runs on a side stream
-        underneath the other half-batch's convolutions.  Data flow per replay: network(A) consumes the leaves lane A
-        selected in the previous replay (or in the prologue wave), k_wave(B) consumes network(B)'s previous output."""
-        A, Bn = self.lanes
-        side = torch.cuda.Stream()
-        cs = torch.cuda.Stream()
-        cs.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(cs):
-            for _ in range(warmup):
-                A.forward(A.nn_in)
-                Bn.forward(Bn.nn_in)
-        torch.cuda.current_stream().wait_stream(cs)
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g, stream=cs):
-            side.wait_stream(cs)
-            with torch.cuda.stream(side):
-                Bn.engine.wave(Bn.nn_in, Bn.logits, Bn.value)
-            A.forward(A.nn_in)
-            cs.wait_stream(side)
-            side.wait_stream(cs)
-            with torch.cuda.stream(side):
-                A.engine.wave(A.nn_in, A.logits, A.value)
-            Bn.forward(Bn.nn_in)
-            cs.wait_stream(side)
-        self.graph = g
-
-    def _search_pipeline(self, m):
-        e = self.engine
-        A, Bn = self.lanes
-        for p in np.unique(self.playouts[m]):
-            e.begin_search(int(p), (m & (self.playouts == p)).astype(np.uint8))
-        pmax = int(self.playouts[m].max()) if m.any() else 0
-        A.engine.wave(A.nn_in, A.logits, A.value)      # prologue: lane A's first leaves
-        waves = 1
-        while True:
-            if self.graph is not None:
-                self.graph.replay()
-                A.engine.launches += 1
-                Bn.engine.launches += 1
-            else:
-                Bn.engine.wave(Bn.nn_in, Bn.logits, Bn.value)
-                A.forward(A.nn_in)
-                A.engine.wave(A.nn_in, A.logits, A.value)
-                Bn.forward(Bn.nn_in)
-            waves += 1
-            if waves > pmax and e.unfinished() == 0:
-                break
-            if waves > 4 * pmax + 64:
-                e.raise_on_error()
-                raise EngineError("search did not converge")
-        self.waves += waves
-        return waves
-
     # -- search_threads = K with row compaction ---------------------------------------------------
     def _eval_rows(self, n):
         """Evaluate the first n rows of the dense batch into logits[:n] / value[:n]."""
@@ -440,93 +298,53 @@ class SelfPlay:
             return self._eval_rows(n)
         g = self._bucket_graphs.get(n)
         if g is None:
-            s = torch.cuda.Stream()
-            s.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(s):
-                for _ in range(2):
-                    self._eval_rows(n)
-            torch.cuda.current_stream().wait_stream(s)
-            torch.cuda.synchronize()
             if self._pool is None:
                 self._pool = torch.cuda.graph_pool_handle()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g, pool=self._pool, stream=torch.cuda.Stream()):
-                self._eval_rows(n)
-            self._bucket_graphs[n] = g
+            g = self._bucket_graphs[n] = capture_cuda_graph(lambda: self._eval_rows(n), lambda: self._eval_rows(n), 2, self._pool)
         g.replay()
-
-    def _search_compact(self, m):
-        e = self.engine
-        if self.plan is not None and hasattr(self.plan, "refresh_if_stale"):
-            self.plan.refresh_if_stale()
-        for p in np.unique(self.playouts[m]):
-            e.begin_search(int(p), (m & (self.playouts == p)).astype(np.uint8))
-        pmax = int(self.playouts[m].max()) if m.any() else 0
-        waves = 0
-        while True:
-            e.wave_compact(self.nn_stage, self.nn_in, self.logits, self.value)
-            n = e.live_rows()                               # stream sync: the host picks the bucket
-            waves += 1
-            if n > 0:
-                self._eval_bucket(n)
-            elif e.unfinished() == 0:                       # nothing to evaluate and every search complete
-                break
-            if waves > 4 * pmax + 64:
-                e.raise_on_error()
-                raise EngineError("search did not converge")
-        self.waves += waves
-        return waves
 
     def capture_graph(self, warmup=3):
         """Capture (wave kernel -> network) into one CUDA graph; the search loop then replays it."""
-        if self.lanes is not None:
-            return self._capture_pipeline(warmup)
         if self.compact:                                    # the wave runs eagerly (the host reads the row count); the network is one
             self._use_graphs = True                         # graph per bucket size, captured on first use
             return
-        s = torch.cuda.Stream()
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):
-            for _ in range(warmup):
-                self._eval(self.nn_in)
-        torch.cuda.current_stream().wait_stream(s)
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        cs = torch.cuda.Stream()
-        with torch.cuda.graph(g, stream=cs):
+
+        def body():
             self.engine.wave(self.nn_in, self.logits, self.value)
             self._eval(self.nn_in)
-        self.graph = g
+        self.graph = capture_cuda_graph(body, lambda: self._eval(self.nn_in), warmup)
 
     def search(self, mask=None):
         """MCTS_tree.main for every live game (or every game with mask[g], e.g. the games where one player of a match is to move):
         `playouts[g]` playouts each."""
         m = self.live if mask is None else np.asarray(mask, dtype=bool)
-        if self.lanes is not None:
-            return self._search_pipeline(m)
-        if self.compact:
-            return self._search_compact(m)
         e = self.engine
         if self.plan is not None and hasattr(self.plan, "refresh_if_stale"):
             self.plan.refresh_if_stale()       # weights trained / restored since the last search (the graph reads them in place)
         for p in np.unique(self.playouts[m]):
             e.begin_search(int(p), (m & (self.playouts == p)).astype(np.uint8))
         pmax = int(self.playouts[m].max()) if m.any() else 0
-        waves = 0
-        while True:
-            if self.graph is not None:
+        if self.compact:
+            n = 0
+
+            def step():
+                nonlocal n
+                e.wave_compact(self.nn_stage, self.nn_in, self.logits, self.value)
+                n = e.live_rows()                           # stream sync: the host picks the bucket
+
+            def evaluate():
+                if n > 0:
+                    self._eval_bucket(n)
+            # done when nothing is left to evaluate and every search is complete
+            waves = run_waves(e, step, 0, pmax, evaluate, may_stop=lambda: n == 0)
+        elif self.graph is not None:
+            def step():
                 self.graph.replay()
                 e.launches += 1          # the captured k_wave launch
-            else:
-                e.wave(self.nn_in, self.logits, self.value)
-            waves += 1
-            if waves > pmax // self.K and e.unfinished() == 0:       # (K leaves per game and wave in the search_threads = K schedule)
-                break
-            if self.graph is None:
-                self._eval(self.nn_in)
-            if waves > 4 * pmax + 64:
-                e.raise_on_error()
-                raise EngineError("search did not converge")
+            waves = run_waves(e, step, pmax // self.K, pmax)
+        else:                            # (K leaves per game and wave in the search_threads = K schedule: pmax // K waves at least)
+            waves = run_waves(e, lambda: e.wave(self.nn_in, self.logits, self.value), pmax // self.K, pmax,
+                              evaluate=lambda: self._eval(self.nn_in))
         self.waves += waves
         return waves
 
@@ -600,8 +418,6 @@ class SelfPlay:
         (Engine.snapshot) and the host state -- boards, sides, live, the per-slot MT19937 states, plies, temperature and each slot's
         unfinished record (its players and log span).  load_games continues exactly where this left off.  The finished games must
         have been handed over with pop_finished first."""
-        if self.lanes is not None:
-            raise ValueError("save_games: the two-lane pipeline cannot be saved")
         if self.finished:
             raise ValueError("save_games: %d finished games were not drained with pop_finished()" % len(self.finished))
         from .train import _savez
@@ -618,8 +434,6 @@ class SelfPlay:
         """Restore what save_games wrote into this SelfPlay (same number of games and engine kind; the engine is restored in place, so
         a captured graph stays valid).  The file is read without pickle and checked; ValueError / EngineError leave everything as it
         was."""
-        if self.lanes is not None:
-            raise ValueError("load_games: the two-lane pipeline cannot be restored")
         with np.load(path, allow_pickle=False) as d:
             a = {k: d[k] for k in d.files}
         B = self.B

@@ -156,10 +156,6 @@ int cz_engine_wave(cz_engine *e, void *stream, void *nn_in, int nn_dtype, const 
 int cz_engine_wave_compact(cz_engine *e, void *stream, void *nn_stage, void *nn_dense, int nn_dtype, const float *logits, const float *value);
 int cz_engine_live_rows(cz_engine *e, void *stream, int32_t *out_rows);
 
-/* the two halves of a wave as separate launches */
-int cz_engine_select(cz_engine *e, void *stream, void *nn_in, int nn_dtype);
-int cz_engine_expand_backup(cz_engine *e, void *stream, const float *logits, const float *value);
-
 /* Board hashing (north_star): when switched on, every wave also leaves the 64-bit Zobrist key of each pending leaf's position
  * (piece-square keys XOR side-to-move key, maintained incrementally along the descent; the root's key lives in the game's header
  * line and is updated by cz_engine_play) in a device array indexed like the network batch rows.  The reference has no position

@@ -117,7 +117,7 @@ def test_fakenets_match_oracle(O, R):
         assert np.array_equal(v.cpu().numpy(), ov.reshape(-1)), kind
 
 
-def _run_cases(cases, net, R, split=False, graph=False, leaves=1):
+def _run_cases(cases, net, R, graph=False, leaves=1):
     """cases: list of dict(board, side, rr, playouts).  Returns the engine after searching."""
     from cchess_zero_b200.engine import Engine
     from cchess_zero_b200.fakenet import FakeNet
@@ -138,11 +138,7 @@ def _run_cases(cases, net, R, split=False, graph=False, leaves=1):
 
     waves = 0
     while True:
-        if split:
-            e.expand_backup(logits, value)
-            e.select(nn_in)
-        else:
-            e.wave(nn_in, logits, value)
+        e.wave(nn_in, logits, value)
         waves += 1
         if e.unfinished() == 0:
             break
@@ -174,14 +170,14 @@ def test_tree_against_reference_vectors(net, R):
         assert got == c["root"], c["note"]
 
 
-@pytest.mark.parametrize("net,split", [("hash_signed", False), ("hash_pos", True)])
-def test_tree_many_positions_vs_oracle(net, split, O, R):
+@pytest.mark.parametrize("net", ["hash_signed", "hash_pos"])
+def test_tree_many_positions_vs_oracle(net, O, R):
     boards, sides = _random_positions(O, 3, 77)
     sel = np.arange(0, len(boards), max(1, len(boards) // 96))[:96]
     rng = np.random.RandomState(1)
     cases = [dict(board=boards[i], side=int(sides[i]), rr=int(rng.choice([0, 5, 56, 58])), playouts=int(rng.choice([50, 150, 250])))
              for i in sel if (boards[i] == 1).any() and (boards[i] == 8).any()]
-    e = _run_cases(cases, net, R, split=split)
+    e = _run_cases(cases, net, R)
     cnt = e.counters()
     tot = dict(n_expand=0, n_playout=0, sum_L=0, sum_c=0)
     for g, c in enumerate(cases):
@@ -235,35 +231,6 @@ def test_selfplay_many_games_vs_oracle(graph, O, R):
         assert np.array_equal(rec.z, r["z"])
         assert np.array_equal(rec.dense_pi(), r["pis"])
         assert rec.actions == r["actions"]
-
-
-def test_two_lane_pipeline_is_bit_exact_vs_oracle(O, R):
-    """The pipelined two-lane schedule (tree kernel of one half under the network of the other) must not change results."""
-    from cchess_zero_b200.fakenet import FakeNet
-    from cchess_zero_b200.selfplay import SelfPlay
-    B, playouts, net = 32, 30, "hash_signed"
-
-    class Plan:
-        def __init__(self, n):
-            self.fn = FakeNet(net)
-        def make_input(self, n):
-            return torch.zeros((n, 9, 10, 14), device="cuda")
-        def __call__(self, x, lo, v):
-            l, val = self.fn(x)
-            lo.copy_(l); v.copy_(val)
-
-    for graph in (False, True):
-        sp = SelfPlay(B, None, playouts, seeds=[500 + i for i in range(B)], arena_words=1 << 20, auto_reset=False,
-                      plan_factory=lambda n: Plan(n), lanes=2)
-        if graph:
-            sp.capture_graph()
-        out = sp.play_games()
-        assert len(out) == B
-        for slot, rec in out:
-            with np.errstate(all="ignore"):
-                r = O.selfplay_game(net, playouts, np.random.RandomState(500 + slot))
-            assert rec.states == r["states"], (graph, slot)
-            assert np.array_equal(rec.dense_pi(), r["pis"]) and np.array_equal(rec.z, r["z"])
 
 
 def test_full_size_1024_games_1200_playouts_properties_and_samples(O, R):
