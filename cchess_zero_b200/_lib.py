@@ -30,6 +30,8 @@ def _sig(L):
     L.cz_encode_batch.argtypes = [i32, vp, vp, i32, vp]
     L.cz_legal_moves_dev.argtypes = [vp, vp, i32, vp, vp, vp]
     L.cz_encode_dev.argtypes = [vp, vp, i32, vp, i32, vp]
+    L.cz_strict_moves_batch.argtypes = [i32, vp, vp, i32, vp, vp, vp, vp]
+    L.cz_strict_moves_dev.argtypes = [vp, vp, i32, vp, vp, vp, vp, vp]
     L.cz_replay_batch.argtypes = [vp, vp, vp, vp, vp, i32, vp, vp, i32, vp, vp, vp, vp]
     L.cz_mirror_labels.argtypes = [vp]
     L.cz_engine_create.argtypes = [i32, i64, i32, C.POINTER(vp)]

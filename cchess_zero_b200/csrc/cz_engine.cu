@@ -1323,6 +1323,25 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) k_legal_moves(const uint
     for (int i = lane; i < CZ_MAXCHILD; i += 32) moves[(size_t)g * CZ_MAXCHILD + i] = i < c ? S.moves[i] : (uint16_t)0;
 }
 
+// k_legal_moves' outputs plus, per position, the 128-bit mask of strictly legal moves and the in-check / mated flags
+// (cz::warp_strict_moves)
+__global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) k_strict_moves(const uint8_t *boards, const uint8_t *sides, int n, uint16_t *moves, int32_t *counts,
+                                                                       uint32_t *legal, uint8_t *flags) {
+    __shared__ WarpSmem smem[WARPS_PER_BLOCK];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, g = blockIdx.x * WARPS_PER_BLOCK + w;
+    if (g >= n) return;
+    WarpSmem &S = smem[w];
+    for (int i = lane; i < 90; i += 32) S.board[i] = boards[(size_t)g * 90 + i];
+    __syncwarp();
+    uint32_t mask[4];
+    int fl;
+    int c = cz::warp_strict_moves(S.board, sides[g], S.moves, S.scratch, lane, mask, fl);
+    if (lane == 0) { counts[g] = c; flags[g] = (uint8_t)fl; }
+    if (lane < 4) legal[(size_t)g * 4 + lane] = lane == 0 ? mask[0] : lane == 1 ? mask[1] : lane == 2 ? mask[2] : mask[3];
+    if (c > CZ_MAXCHILD) c = CZ_MAXCHILD;
+    for (int i = lane; i < CZ_MAXCHILD; i += 32) moves[(size_t)g * CZ_MAXCHILD + i] = i < c ? S.moves[i] : (uint16_t)0;
+}
+
 template <typename T>
 __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) k_encode(const uint8_t *boards, const uint8_t *sides, int n, T *out) {
     __shared__ WarpSmem smem[WARPS_PER_BLOCK];
@@ -1563,6 +1582,14 @@ int cz_legal_moves_dev(const uint8_t *boards, const uint8_t *sides, int n, uint1
     return CZ_OK;
 }
 
+int cz_strict_moves_dev(const uint8_t *boards, const uint8_t *sides, int n, uint16_t *moves, int32_t *counts, uint32_t *legal, uint8_t *flags,
+                        void *stream) {
+    if (n <= 0) return CZ_OK;
+    k_strict_moves<<<nblk(n, WARPS_PER_BLOCK), 32 * WARPS_PER_BLOCK, 0, (cudaStream_t)stream>>>(boards, sides, n, moves, counts, legal, flags);
+    CUDA_TRY(cudaGetLastError());
+    return CZ_OK;
+}
+
 int cz_encode_dev(const uint8_t *boards, const uint8_t *sides, int n, void *out, int dtype, void *stream) {
     if (n <= 0) return CZ_OK;
     dim3 gr(nblk(n, WARPS_PER_BLOCK)), bl(32 * WARPS_PER_BLOCK);
@@ -1615,6 +1642,30 @@ int cz_legal_moves_batch(int device, const uint8_t *boards, const uint8_t *sides
     if (rc) return rc;
     CUDA_TRY(cudaMemcpy(moves, dm, (size_t)n * CZ_MAXCHILD * 2, cudaMemcpyDeviceToHost));
     CUDA_TRY(cudaMemcpy(counts, dc, (size_t)n * 4, cudaMemcpyDeviceToHost));
+    return CZ_OK;
+}
+
+int cz_strict_moves_batch(int device, const uint8_t *boards, const uint8_t *sides, int n, uint16_t *moves, int32_t *counts, uint32_t *legal,
+                          uint8_t *flags) {
+    if (n < 0 || (n && (!boards || !sides || !moves || !counts || !legal || !flags))) return fail(CZ_EINVAL, "cz_strict_moves_batch: null");
+    if (n == 0) return CZ_OK;
+    DevBufs bufs;
+    uint8_t *db = nullptr, *ds = nullptr, *df = nullptr;
+    uint16_t *dm = nullptr;
+    int32_t *dc = nullptr;
+    uint32_t *dl = nullptr;
+    int rc = batch_io(bufs, device, boards, sides, n, &db, &ds);
+    if (rc) return rc;
+    CUDA_TRY(bufs.alloc(&dm, (size_t)n * CZ_MAXCHILD * 2));
+    CUDA_TRY(bufs.alloc(&dc, (size_t)n * 4));
+    CUDA_TRY(bufs.alloc(&dl, (size_t)n * 16));
+    CUDA_TRY(bufs.alloc(&df, (size_t)n));
+    rc = cz_strict_moves_dev(db, ds, n, dm, dc, dl, df, nullptr);
+    if (rc) return rc;
+    CUDA_TRY(cudaMemcpy(moves, dm, (size_t)n * CZ_MAXCHILD * 2, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(counts, dc, (size_t)n * 4, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(legal, dl, (size_t)n * 16, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(flags, df, (size_t)n, cudaMemcpyDeviceToHost));
     return CZ_OK;
 }
 

@@ -179,6 +179,119 @@ CZ_HD void bits_from_board(const uint8_t *b, Bits &P) {
     }
 }
 
+// ---- strict legality ---------------------------------------------------------------------------------------------
+// in_check(board, side): some pseudo-legal move of the OTHER side, as gen_piece_bits / kings_face list them, ends on the
+// square of `side`'s king (false when that king is absent).  A pseudo-legal move is strictly legal iff the mover is not in
+// check after it.  No replies are generated: `attacked` asks, from the king's square, where each kind of attacker would
+// have to stand, with the attacker's own placement rules exactly as gen_piece_bits applies them to its targets.
+
+// The position after moving src -> dst, never materialised: the bitboards are patched in registers and a piece is looked up
+// as "dst holds what stood on src, src is empty, everything else is the board b".  src = dst = -1 is the board itself.
+struct Moved {
+    const uint8_t *b;
+    int src, dst;
+    CZ_HD int at(int s) const { return s == dst ? b[src] : s == src ? 0 : b[s]; }
+};
+
+CZ_HD void bb_put(uint32_t (&w)[3], int s, bool v) {
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        const uint32_t m = (s >> 5) == k ? 1u << (s & 31) : 0u;
+        w[k] = v ? (w[k] | m) : (w[k] & ~m);
+    }
+}
+
+// P after the piece on src (of colour mover_red) moved to dst; a capture needs no extra step
+CZ_HD Bits bits_after(const Bits &P, int src, int dst, bool mover_red) {
+    Bits Q = P;
+    bb_put(Q.occ, src, false); bb_put(Q.red, src, false); bb_put(Q.rocc, (src % 9) * 10 + src / 9, false);
+    bb_put(Q.occ, dst, true); bb_put(Q.red, dst, mover_red); bb_put(Q.rocc, (dst % 9) * 10 + dst / 9, true);
+    return Q;
+}
+
+// Is the king of `side` on ksq attacked in the position (P, M)?  esq: the other king's square or -1.
+CZ_HD bool attacked(const Bits &P, const Moved &M, int side, int ksq, int esq) {
+    const int foe = side == 0 ? 7 : 0;                  // piece code of an attacker of kind k is k + foe
+    const bool foe_red = side != 0;
+    const int y = ksq / 9, x = ksq - y * 9;
+    // rook = first piece met along the rank / file, cannon = second
+    const uint32_t rank = bb_line(P.occ, y * 9, 9), file = bb_line(P.rocc, x * 10, 10);
+#pragma unroll 1
+    for (int d = 0; d < 4; d++) {
+        const bool horiz = d < 2, fwd = d & 1;
+        const uint32_t line = horiz ? rank : file;
+        const int pos = horiz ? x : y, step = horiz ? 1 : 9, base = horiz ? y * 9 : x;
+        int first = -1, second = -1;
+        if (fwd) {
+            uint32_t m = line >> (pos + 1);
+            if (m) { first = pos + 1 + bb_lsb(m); m &= m - 1; if (m) second = pos + 1 + bb_lsb(m); }
+        } else {
+            uint32_t m = line & ((1u << pos) - 1u);
+            if (m) { first = bb_msb(m); m &= ~(1u << first); if (m) second = bb_msb(m); }
+        }
+        if (first >= 0 && M.at(base + first * step) == R_ + foe) return true;
+        if (second >= 0 && M.at(base + second * step) == C_ + foe) return true;
+    }
+    // knight: both knight squares beyond a diagonal neighbour share it as their leg (the square next to the knight)
+#pragma unroll
+    for (int ij = 0; ij < 4; ij++) {
+        const int i = (ij & 2) ? 1 : -1, j = (ij & 1) ? 1 : -1;
+        const int ly = y + i, lx = x + j;
+        if (ly < 0 || ly > 9 || lx < 0 || lx > 8 || bb_test(P.occ, ly * 9 + lx)) continue;
+        if (y + 2 * i >= 0 && y + 2 * i <= 9 && M.at((y + 2 * i) * 9 + lx) == N_ + foe) return true;
+        if (x + 2 * j >= 0 && x + 2 * j <= 8 && M.at(ly * 9 + x + 2 * j) == N_ + foe) return true;
+    }
+    // pawn: from behind (its forward step), and from either side once it stands beyond its river
+    {
+        const int py = foe_red ? y - 1 : y + 1;
+        if (py >= 0 && py <= 9 && M.at(py * 9 + x) == P_ + foe) return true;
+        if (foe_red ? y > 4 : y < 5) {
+            if (x > 0 && M.at(ksq - 1) == P_ + foe) return true;
+            if (x < 8 && M.at(ksq + 1) == P_ + foe) return true;
+        }
+    }
+    // bishop: two diagonal steps with an empty eye; it only lands in its own half
+    if (foe_red ? y <= 4 : y >= 5) {
+#pragma unroll
+        for (int ij = 0; ij < 4; ij++) {
+            const int i = (ij & 2) ? 1 : -1, j = (ij & 1) ? 1 : -1;
+            const int by = y + 2 * i, bx = x + 2 * j;
+            if (by < 0 || by > 9 || bx < 0 || bx > 8) continue;
+            if (!bb_test(P.occ, (y + i) * 9 + x + j) && M.at(by * 9 + bx) == B_ + foe) return true;
+        }
+    }
+    // advisor and the king's palace step: they only land inside their own palace
+    if (x >= 3 && x <= 5 && (foe_red ? y <= 2 : y >= 7)) {
+#pragma unroll
+        for (int ij = 0; ij < 4; ij++) {
+            const int ay = y + ((ij & 2) ? 1 : -1), ax = x + ((ij & 1) ? 1 : -1);
+            if (ay >= 0 && ay <= 9 && ax >= 0 && ax <= 8 && M.at(ay * 9 + ax) == A_ + foe) return true;
+        }
+        if (esq >= 0) {
+            const int ey = esq / 9, ex = esq - ey * 9;
+            if ((ey == y && (ex == x - 1 || ex == x + 1)) || (ex == x && (ey == y - 1 || ey == y + 1))) return true;
+        }
+    }
+    // flying general, the same test that appends the capture to the move list
+    return side == 0 ? kings_face(P, ksq, esq) : kings_face(P, esq, ksq);
+}
+
+// in_check of the board itself.  Ksq / ksq: the king squares (-1 if absent).
+CZ_HD bool in_check(const Bits &P, const uint8_t *b, int side, int Ksq, int ksq) {
+    const int mine = side == 0 ? Ksq : ksq, other = side == 0 ? ksq : Ksq;
+    return mine >= 0 && attacked(P, Moved{b, -1, -1}, side, mine, other);
+}
+
+// Is the pseudo-legal move mv of `side` strictly legal on (P, b)?
+CZ_HD bool move_is_strict(const Bits &P, const uint8_t *b, int side, int mv, int Ksq, int ksq) {
+    const int src = mv & 127, dst = (mv >> 7) & 127;
+    int mine = side == 0 ? Ksq : ksq, other = side == 0 ? ksq : Ksq;
+    if (src == mine) mine = dst;                        // the king itself moves
+    if (dst == other) other = -1;                       // the other king is captured
+    if (mine < 0) return true;
+    return !attacked(bits_after(P, src, dst, side == 0), Moved{b, src, dst}, side, mine, other);
+}
+
 #ifdef __CUDACC__
 __device__ __forceinline__ int warp_excl_scan(int v, int lane, int &total) {
     int inc = v;
@@ -251,6 +364,28 @@ __device__ __noinline__ int warp_legal_moves(const uint8_t *b, int side, uint16_
         n++;
     }
     __syncwarp();
+    return n;
+}
+
+// warp_legal_moves (same list, order and count) plus strict legality: bit i of the 128-bit legal mask is set iff move i
+// leaves the mover's king unattacked (bits at and above min(count, 128) are zero); flags bit 0 = the mover is in check,
+// bit 1 = mated (no strictly legal move: checkmate or stalemate).  Lane l tests moves l, l + 32, l + 64, l + 96, each
+// against bitboards patched in its own registers; nothing but the mailbox b is read.  All 32 lanes must call, converged.
+__device__ __forceinline__ int warp_strict_moves(const uint8_t *b, int side, uint16_t *moves, MoveScratch &T, int lane,
+                                                 uint32_t (&legal)[4], int &flags) {
+    const int n = warp_legal_moves(b, side, moves, T, lane);
+    Bits P;
+    int Ksq, ksq;
+    warp_bits(b, lane, P, Ksq, ksq);
+    uint32_t any = 0;
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+        const int i = lane + 32 * k;
+        const bool ok = i < n && move_is_strict(P, b, side, moves[i], Ksq, ksq);
+        legal[k] = __ballot_sync(CZ_FULL, ok);
+        any |= legal[k];
+    }
+    flags = (in_check(P, b, side, Ksq, ksq) ? 1 : 0) | (any ? 0 : 2);
     return n;
 }
 #endif  // __CUDACC__

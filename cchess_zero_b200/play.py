@@ -13,7 +13,7 @@ class ChessGame(object):
     """Text-mode stand-in for the reference's ChessGame: same constructor arguments, start()/perform_AI()/change_player()."""
 
     def __init__(self, in_ai_count, in_ai_function, in_play_playout, in_delay=0.0, in_end_delay=0.0, batch_size=128, search_threads=16,
-                 processor="gpu", num_gpus=1, res_block_nums=7, human_color="b", network=None, quiet=False):
+                 processor="gpu", num_gpus=1, res_block_nums=7, human_color="b", network=None, quiet=False, strict=False):
         self.ai_count, self.ai_function = in_ai_count, in_ai_function
         self.delay, self.end_delay, self.quiet = in_delay, in_end_delay, quiet
         self.current_player = "w"
@@ -21,7 +21,7 @@ class ChessGame(object):
         self.move_times = []
         self.cchess_engine = cchess_main(playout=in_play_playout, in_batch_size=batch_size, exploration=False, in_search_threads=search_threads,
                                          processor=processor, num_gpus=num_gpus, res_block_nums=res_block_nums, human_color=human_color,
-                                         network=network, log_file=False)
+                                         network=network, log_file=False, strict=strict)
 
     def perform_AI(self):  # ChessGame.py:183-195
         t0 = time.perf_counter()
@@ -42,7 +42,13 @@ class ChessGame(object):
                 self.perform_AI()
             else:
                 coord = tuple(int(t) for t in input("move (x0 y0 x1 y1): ").split())
-                self.cchess_engine.human_move(coord, self.ai_function)
+                try:
+                    self.cchess_engine.human_move(coord, self.ai_function)
+                except ValueError as e:      # strict rules: the move would leave the king attacked; ask again
+                    if not self.cchess_engine.strict:
+                        raise
+                    print(e)
+                    continue
             n += 1
             if self.delay:
                 time.sleep(self.delay)
@@ -58,7 +64,8 @@ def main():
     ap.add_argument("--res_block_nums", default=7, type=int)
     ap.add_argument("--human_color", default="b", choices=["w", "b"])
     a = ap.parse_args()
-    g = ChessGame(a.ai_count, a.ai_function, a.play_playout, a.delay, res_block_nums=a.res_block_nums, human_color=a.human_color)
+    # a human at the terminal expects the full rules: no self-check, mate ends the game
+    g = ChessGame(a.ai_count, a.ai_function, a.play_playout, a.delay, res_block_nums=a.res_block_nums, human_color=a.human_color, strict=True)
     print("result:", g.start())
 
 

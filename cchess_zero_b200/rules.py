@@ -101,6 +101,22 @@ def legal_moves_batch(boards, sides):
     return mv, cnt
 
 
+def strict_moves_batch(boards, sides):
+    """legal_moves_batch plus strict legality (cz_strict_moves_batch, one launch): -> (moves, counts, legal bool [n, 128],
+    in_check bool [n], mated bool [n]).  legal[g, i]: move i does not leave the mover's king attacked (flying general included);
+    mated: no such move, checkmate or stalemate."""
+    boards = np.ascontiguousarray(boards, dtype=np.uint8).reshape(-1, 90)
+    sides = np.ascontiguousarray(sides, dtype=np.uint8)
+    n = boards.shape[0]
+    mv = np.zeros((n, MAXCHILD), dtype=np.uint16)
+    cnt = np.zeros(n, dtype=np.int32)
+    mask = np.zeros((n, 4), dtype=np.uint32)
+    flags = np.zeros(n, dtype=np.uint8)
+    check(lib().cz_strict_moves_batch(_device(), _hp(boards), _hp(sides), n, _hp(mv), _hp(cnt), _hp(mask), _hp(flags)), "cz_strict_moves_batch")
+    legal = ((mask[:, :, None] >> np.arange(32, dtype=np.uint32)) & 1).astype(bool).reshape(n, MAXCHILD)
+    return mv, cnt, legal, (flags & 1).astype(bool), (flags & 2).astype(bool)
+
+
 def apply_moves_batch(boards, moves):
     boards = np.array(boards, dtype=np.uint8, copy=True).reshape(-1, 90)
     moves = np.ascontiguousarray(moves, dtype=np.uint16)
@@ -182,3 +198,14 @@ class GameBoard(object):
         """main.py:743-1109 -> cz_legal_moves_batch (n = 1); same move order."""
         mv, cnt = legal_moves_batch(state_to_board(state)[None], [side_of(current_player)])
         return [move_to_label(m) for m in mv[0, : cnt[0]]]
+
+    @staticmethod
+    def get_strict_moves(state, current_player):
+        """The moves of get_legal_moves, in the same order, that do not leave the mover's own king attacked."""
+        mv, cnt, legal, _, _ = strict_moves_batch(state_to_board(state)[None], [side_of(current_player)])
+        return [move_to_label(m) for m, ok in zip(mv[0, : cnt[0]], legal[0]) if ok]
+
+    @staticmethod
+    def in_check(state, current_player):
+        """Could the other side capture current_player's king if it were to move (flying general included)?"""
+        return bool(strict_moves_batch(state_to_board(state)[None], [side_of(current_player)])[3][0])

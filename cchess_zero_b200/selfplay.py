@@ -523,9 +523,14 @@ def load_replay(path, restore_rng=True):
 
 
 class cchess_main(object):
+    # strict=True plays by the full rules of xiangqi instead of the reference's (pseudo-legal moves, the game ends when a king is
+    # captured): no move that leaves the own king attacked or is in banned_moves is played, a mated side has lost, and
+    # human_move refuses such a move.  The search is the same either way; the filter is applied to its result.
+    strict = False
+    banned_moves = ()       # move labels the next get_action / select_move must not play (a GUI's perpetual-check ban)
 
     def __init__(self, playout=400, in_batch_size=128, exploration=True, in_search_threads=16, processor="cpu",
-                 num_gpus=1, res_block_nums=7, human_color="b", network=None, log_file=True, leaf_parallel=1):
+                 num_gpus=1, res_block_nums=7, human_color="b", network=None, log_file=True, leaf_parallel=1, strict=False):
         from .mcts import MCTS_tree
         from .net import policy_value_network, policy_value_network_gpus
         rules._init_tables()
@@ -554,6 +559,7 @@ class cchess_main(object):
         self.kl_targ = 0.025
         self.log_file = open(os.path.join(os.getcwd(), "log_file.txt"), "w") if log_file else None
         self.human_color = human_color
+        self.strict = strict
 
     @staticmethod
     def flip_policy(prob):  # main.py:1152-1155
@@ -658,14 +664,47 @@ class cchess_main(object):
             tot_p += mov_p
         return moves, [x / tot_p for x in p], value
 
+    # ---- strict legality (strict=True only) ----------------------------------------------------------
+    def _strict_position(self):
+        """(pseudo-legal move labels, their strict-legality flags, in check, mated) for the side to move on the board:
+        one k_strict_moves launch."""
+        gb = self.game_borad
+        mv, cnt, legal, chk, mated = rules.strict_moves_batch(rules.state_to_board(gb.state)[None], [rules.side_of(gb.current_player)])
+        n = min(int(cnt[0]), mv.shape[1])
+        return [rules.move_to_label(m) for m in mv[0, :n]], legal[0, :n], bool(chk[0]), bool(mated[0])
+
+    def _playable(self):
+        """Labels of the moves that are strictly legal and not banned."""
+        labels, legal, _, _ = self._strict_position()
+        return {m for m, ok in zip(labels, legal) if ok and m not in self.banned_moves}
+
+    def _strict_visits(self, actions, visits):
+        """The root's visit counts with every child that may not be played set to 0.  When no playable child was visited, the
+        playable child with the largest prior gets the only visit (first maximum wins)."""
+        playable = self._playable()
+        kept = tuple(v if a in playable else 0 for a, v in zip(actions, visits))
+        if any(kept):
+            return kept
+        rest = [a for a in actions if a in playable]
+        if not rest:
+            raise ValueError("no move is both strictly legal and not banned")
+        child = self.mcts.root.child
+        best = max(rest, key=lambda a: child[a].P)
+        return tuple(1 if a == best else 0 for a in actions)
+
     def get_action(self, state, temperature=1e-3):
         self.mcts.main(state, self.game_borad.current_player, self.game_borad.restrict_round, self.playout_counts)
         actions_visits = [(act, nod.N) for act, nod in self.mcts.root.child.items()]
         actions, visits = zip(*actions_visits)
+        if self.strict:
+            visits = self._strict_visits(actions, visits)
         with np.errstate(divide="ignore"):
             probs = rules.softmax(1.0 / temperature * np.log(visits))
         move_probs = [[actions, probs]]
-        if self.exploration:
+        if self.exploration and self.strict:      # the Dirichlet noise must not revive a filtered move
+            p = np.where(np.asarray(visits) > 0, 0.75 * probs + 0.25 * np.random.dirichlet(0.3 * np.ones(len(probs))), 0.0)
+            act = np.random.choice(actions, p=p / p.sum())
+        elif self.exploration:
             act = np.random.choice(actions, p=0.75 * probs + 0.25 * np.random.dirichlet(0.3 * np.ones(len(probs))))
         else:
             act = np.random.choice(actions, p=probs)
@@ -685,6 +724,12 @@ class cchess_main(object):
         elif self.game_borad.restrict_round >= 60:
             print("TIE! No Winners!")
             return True, "t"
+        elif self.strict and self._strict_position()[3]:      # checkmate or stalemate: the side to move has lost
+            if self.game_borad.current_player == "w":
+                print("Green is Winner")
+                return True, "b"
+            print("Red is Winner")
+            return True, "w"
         return False, ""
 
     def _advance(self, action):
@@ -703,6 +748,10 @@ class cchess_main(object):
         action = "abcdefghi"[coord[0]] + str(coord[1]) + "abcdefghi"[coord[2]] + str(coord[3])
         if self.human_color == "w":
             action = "".join(rules.flipped_uci_labels(action))
+        if self.strict:
+            labels, legal, _, _ = self._strict_position()
+            if action not in {m for m, ok in zip(labels, legal) if ok}:
+                raise ValueError("%s is not a legal move" % action)
         if mcts_or_net == "mcts":
             if self.mcts.root.child == {}:
                 self.mcts.main(self.game_borad.state, self.game_borad.current_player, self.game_borad.restrict_round, self.playout_counts)
@@ -717,6 +766,9 @@ class cchess_main(object):
         else:
             moves, p, value = self._net_priors()
             win_rate = value[0, 0]
+            if self.strict:
+                playable = self._playable()
+                moves, p = zip(*[(m, q) for m, q in zip(moves, p) if m in playable])
             action = max(zip(moves, p), key=lambda t: t[1])[0]   # first maximum wins, main.py:1461
         print("Win rate for player {} is {:.4f}".format(self.game_borad.current_player, win_rate))
         print(self.game_borad.current_player, " now take a action : ", action, "[Step {}]".format(self.game_borad.round))

@@ -4,7 +4,7 @@ Universal Chinese Chess Interface text protocol instead of the reference's tkint
     python -m cchess_zero_b200.ucci [--playouts 1200] [--res_block_nums 7] [--leaf_parallel 8]
 
 Commands understood: ucci, isready, setoption name <playouts|leaf_parallel|temperature> value <v>, position {startpos | fen <fen>}
-[moves m1 m2 ...], banmoves (ignored), go [nodes N | depth D | time ms ...] (nodes = playouts; depth/time are accepted and
+[moves m1 m2 ...], banmoves m1 m2 ... (the next go does not play them; the next position clears them), go [nodes N | depth D | time ms ...] (nodes = playouts; depth/time are accepted and
 ignored -- the reference searches a fixed playout count, main.py:1336), stop (no-op: go is synchronous like the reference's
 blocking forward), probe/d (print position), quit.
 
@@ -13,7 +13,9 @@ Coordinates: UCCI squares are file a-i, rank 0-9 counted from Red's back rank --
 starts at rank 0 (main.py:585), so the rows are reversed; H/E are accepted as aliases of N/B.
 
 The search object is injected (`driver`): anything with cchess_main's attributes `game_borad`, `mcts`, `playout_counts`,
-`get_action`, `check_end` -- tests drive the protocol on CPU with a stand-in, the module's main() builds the real one."""
+`get_action`, `check_end`, `banned_moves` -- tests drive the protocol on CPU with a stand-in, the module's main() builds the real
+one with strict=True: it never answers with a move that leaves its own king attacked, and answers nobestmove when it is mated.
+main() also checks the moves of `position` for strict legality (`legal_moves`) and refuses a list that holds an illegal one."""
 import sys
 
 START_STATE = "RNBAKABNR/9/1C5C1/P1P1P1P1P/9/9/p1p1p1p1p/1c5c1/9/rnbakabnr"
@@ -105,8 +107,11 @@ class UcciEngine:
 
     NAME = "cchess-zero-b200"
 
-    def __init__(self, driver_factory, out=None, playouts=1200, leaf_parallel=1):
+    def __init__(self, driver_factory, out=None, playouts=1200, leaf_parallel=1, legal_moves=None):
+        """legal_moves: (state, player) -> [move labels]; when given, every move of a `position` command must be in it."""
         self._factory = driver_factory
+        self._legal_moves = legal_moves
+        self._banned = ()
         self._driver = None
         self.out = out if out is not None else sys.stdout
         self.options = {"playouts": int(playouts), "leaf_parallel": int(leaf_parallel), "temperature": 1e-3}
@@ -203,12 +208,15 @@ class UcciEngine:
         else:
             raise UcciError("position needs startpos or fen")
         state, player, rr = base
-        for m in moves:                                   # validate before committing
+        for k, m in enumerate(moves):                     # validate before committing
+            if self._legal_moves is not None and m not in self._legal_moves(state, player):
+                raise UcciError("illegal move %s (move %d)" % (m, k + 1))
             state, _ = apply_move(state, m)
-        self._base, self._moves = base, moves
+            player = "b" if player == "w" else "w"
+        self._base, self._moves, self._banned = base, moves, ()
 
     def cmd_banmoves(self, args):
-        pass
+        self._banned = tuple(parse_move(m) for m in args)
 
     def cmd_go(self, args):
         playouts = self.options["playouts"]
@@ -216,12 +224,20 @@ class UcciEngine:
             playouts = int(args[args.index("nodes") + 1])
         d = self._sync()
         d.playout_counts = playouts
+        d.banned_moves = self._banned
         ended, who = d.check_end()
         if ended:
             self._say("info string game over (%s)" % who)
             self._say("nobestmove")
             return
-        act, move_probs, win_rate = d.get_action(d.game_borad.state, self.options["temperature"])
+        try:
+            act, move_probs, win_rate = d.get_action(d.game_borad.state, self.options["temperature"])
+        except ValueError as e:                           # strict rules: every legal move is banned
+            if not getattr(d, "strict", False):
+                raise
+            self._say("info string %s" % e)
+            self._say("nobestmove")
+            return
         # get_action already re-rooted the tree on `act` (main.py:1351); mirror it in the protocol state so that the GUI's next
         # "position ... moves ... act reply" continues inside the same tree.
         state, player, rr, rnd = self._position_now()
@@ -274,7 +290,7 @@ def _real_driver(res_block_nums):
     def make(options):
         from .selfplay import cchess_main
         return cchess_main(playout=options["playouts"], exploration=False, processor="gpu", res_block_nums=res_block_nums,
-                           log_file=False, leaf_parallel=options["leaf_parallel"])
+                           log_file=False, leaf_parallel=options["leaf_parallel"], strict=True)
     return make
 
 
@@ -286,7 +302,9 @@ def main():
     ap.add_argument("--leaf_parallel", default=8, type=int)
     ap.add_argument("--res_block_nums", default=7, type=int)
     a = ap.parse_args()
-    eng = UcciEngine(_real_driver(a.res_block_nums), out=sys.stdout, playouts=a.playouts, leaf_parallel=a.leaf_parallel)
+    from .rules import GameBoard
+    eng = UcciEngine(_real_driver(a.res_block_nums), out=sys.stdout, playouts=a.playouts, leaf_parallel=a.leaf_parallel,
+                     legal_moves=GameBoard.get_strict_moves)
     real_out = sys.stdout
     eng.out = real_out
     with contextlib.redirect_stdout(sys.stderr):      # cchess_main prints progress lines; keep the protocol stream clean

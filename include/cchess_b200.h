@@ -78,6 +78,24 @@ int cz_encode_batch(int device, const uint8_t *boards, const uint8_t *sides, int
 int cz_legal_moves_dev(const uint8_t *boards, const uint8_t *sides, int n, uint16_t *moves, int32_t *counts, void *stream);
 int cz_encode_dev(const uint8_t *boards, const uint8_t *sides, int n, void *out, int dtype, void *stream);
 
+/* ---- strict legality (no counterpart in the reference, whose moves are pseudo-legal and whose games end by king capture) ----
+ * in_check(board, side): some pseudo-legal move of the other side, flying general included, ends on side's king (false when
+ * that king is absent).  A pseudo-legal move is strictly legal iff the mover is not in check after it; a side without a
+ * strictly legal move is mated (checkmate or stalemate, both lose).  Boards may be any placement with at most one king per colour.
+ * Per position:  moves / counts  exactly what cz_legal_moves_batch writes for the same input (a count above CZ_MAXCHILD is
+ *                                returned as it is and the list is truncated);
+ *                legal u32[4]    bit i & 31 of word i >> 5 is set iff move i is strictly legal; bits at and above
+ *                                min(count, 128) are zero;
+ *                flags u8        bit 0 (CZ_IN_CHECK) = in_check(board, side), bit 1 (CZ_MATED) = no strictly legal move.
+ * The batch form takes host buffers (null / n < 0 -> CZ_EINVAL, n == 0 -> CZ_OK); the dev form takes device pointers, launches
+ * on `stream`, and neither allocates nor synchronises. */
+#define CZ_IN_CHECK 1
+#define CZ_MATED 2
+int cz_strict_moves_batch(int device, const uint8_t *boards /* [n][90] */, const uint8_t *sides /* [n] */, int n,
+                          uint16_t *moves /* [n][128] */, int32_t *counts /* [n] */, uint32_t *legal /* [n][4] */, uint8_t *flags /* [n] */);
+int cz_strict_moves_dev(const uint8_t *boards, const uint8_t *sides, int n, uint16_t *moves, int32_t *counts, uint32_t *legal,
+                        uint8_t *flags, void *stream);
+
 /* ---- replay buffer -> training mini-batch (cchess_main.policy_update's data path, main.py:1160-1166 + run() 1236-1239) ----
  * The ring holds cap records in device arrays: boards u8 [cap][90] (side-to-move canonical), n u8 [cap], idx i16 [cap][128]
  * (label indices), prob f32 [cap][128] (visit probabilities), z f32 [cap].  Output row r is ring record rows[r]:
