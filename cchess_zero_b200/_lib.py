@@ -9,6 +9,8 @@ LIB_PATH = os.path.join(_HERE, "libcchess_b200.so")
 NSQ, NLABEL, MAXCHILD, ENC_LEN, STATUS_BYTES, MT_WORDS = 90, 2086, 128, 1260, 112, 626
 F32, BF16, F16, BOARD = 0, 1, 2, 3
 ERR_NAMES = {1: "NOMOVES", 2: "NOLABEL", 4: "DEPTH", 8: "ARENA", 16: "CHILDREN", 32: "ILLEGAL"}
+RULES = {"reference": 0, "strict": 1}     # CZ_RULES_REFERENCE / CZ_RULES_STRICT
+TERM_MATED = 3                            # terminal code of a game whose side to move has no strictly legal move (strict engines)
 
 _lib = None
 
@@ -39,6 +41,8 @@ def _sig(L):
     L.cz_engine_create_fifo.argtypes = [i32, i64, i32, i32, C.POINTER(vp)]
     L.cz_engine_is_fifo.argtypes = [vp]
     L.cz_engine_leaves.argtypes = [vp]
+    L.cz_engine_create_rules.argtypes = [i32, i64, i32, i32, C.POINTER(vp)]
+    L.cz_engine_rules.argtypes = [vp]
     L.cz_engine_destroy.argtypes = [vp]
     L.cz_engine_n_games.argtypes = [vp]
     L.cz_engine_reset.argtypes = [vp, vp, vp, vp, vp, vp]
@@ -64,6 +68,7 @@ def _sig(L):
     L.cz_engine_snapshot.argtypes = [vp, vp, vp, i64, vp]
     L.cz_engine_restore.argtypes = [vp, vp, vp, i64]
     L.cz_snapshot_check.argtypes = [vp, i64, i32, i32, i32, i64]
+    L.cz_snapshot_check_rules.argtypes = [vp, i64, i32, i32, i32, i64, i32]
     L.cz_net_first_conv.argtypes = [vp, i32, vp, vp, vp, vp]
     L.cz_net_heads.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.cz_host_choose_moves.argtypes = [i32, vp, vp, vp, i32, vp, vp, vp, vp, i32]

@@ -21,8 +21,9 @@ import sys
 import numpy as np
 import torch
 
-from . import rules
-from ._lib import MT_WORDS, NLABEL, EngineError
+from . import rules as _rules                        # (random_openings and Match take a `rules` argument)
+from ._lib import MT_WORDS, NLABEL, TERM_MATED, EngineError
+from .engine import check_rules
 from .selfplay import SelfPlay, network_selfplay, sample_moves
 
 NO_MOVE = 0xFFFF
@@ -39,11 +40,14 @@ class UniformEvaluator:
         return torch.zeros((n, NLABEL), dtype=torch.float32, device=x.device), torch.zeros((n,), dtype=torch.float32, device=x.device)
 
 
-def random_openings(n_pairs, plies, seed=0):
+def random_openings(n_pairs, plies, seed=0, rules="reference"):
     """n_pairs start positions reached by `plies` uniformly random legal moves from the start position (positions where a king was
-    captured are drawn again).  -> (boards u8 [n_pairs, 90], sides u8 [n_pairs], restrict_round i32 [n_pairs])."""
+    captured are drawn again).  -> (boards u8 [n_pairs, 90], sides u8 [n_pairs], restrict_round i32 [n_pairs]).
+    rules='strict': the moves are drawn from the strictly legal ones, and an opening that reaches a position without one (mated) is
+    drawn again, so every opening is a running game under the strict rules."""
+    strict = check_rules(rules) == "strict"
     rs = np.random.RandomState(seed)
-    start = rules.state_to_board(rules.START_STATE)
+    start = _rules.state_to_board(_rules.START_STATE)
     boards = np.tile(start, (n_pairs, 1))
     sides = np.zeros(n_pairs, dtype=np.uint8)
     rr = np.zeros(n_pairs, dtype=np.int32)
@@ -56,13 +60,20 @@ def random_openings(n_pairs, plies, seed=0):
         r = np.zeros(len(todo), dtype=np.int32)
         dead = np.zeros(len(todo), dtype=bool)
         for _ in range(plies):
-            mv, cnt = rules.legal_moves_batch(b, s)
+            if strict:                                   # the strictly legal moves, compacted in move-generation order
+                mv, cnt, legal, _, _ = _rules.strict_moves_batch(b, s)
+                order = np.argsort(~legal, axis=1, kind="stable")
+                mv, cnt = np.take_along_axis(mv, order, axis=1), legal.sum(axis=1).astype(np.int32)
+            else:
+                mv, cnt = _rules.legal_moves_batch(b, s)
             dead |= cnt <= 0
             pick = rs.randint(0, np.maximum(cnt, 1))
-            b, cap = rules.apply_moves_batch(b, mv[np.arange(len(todo)), pick])
+            b, cap = _rules.apply_moves_batch(b, mv[np.arange(len(todo)), pick])
             dead |= (cap == 1) | (cap == 8)
             r = np.where(cap == 0, r + 1, 0).astype(np.int32)
             s ^= 1
+        if strict:
+            dead |= _rules.strict_moves_batch(b, s)[4]
         ok = ~dead
         boards[todo[ok]], sides[todo[ok]], rr[todo[ok]] = b[ok], s[ok], r[ok]
         todo = todo[dead]
@@ -125,9 +136,9 @@ class MatchResult:
 class _Player:
     """One player's trees of one half of the games: an engine driven by a SelfPlay used for its search() only."""
 
-    def __init__(self, evaluator, n, playouts, search_threads, arena_words, colour, lo):
+    def __init__(self, evaluator, n, playouts, search_threads, arena_words, colour, lo, rules="reference"):
         self.colour, self.lo, self.hi = colour, lo, lo + n
-        kw = dict(auto_reset=False, keep_records=False, search_threads=search_threads, arena_words=arena_words)
+        kw = dict(auto_reset=False, keep_records=False, search_threads=search_threads, arena_words=arena_words, rules=rules)
         if hasattr(evaluator, "native_plan"):                       # a policy_value_network: its own plan and precision
             self.sp = network_selfplay(evaluator, n, playouts, **kw)
         else:                                                       # a device callable (nn_in) -> (logits, value)
@@ -140,26 +151,30 @@ class Match:
     """candidate vs best over n_games concurrent games; step() plays one ply of every running game, run() plays them all out."""
 
     def __init__(self, candidate, best, n_games, playouts, search_threads=1, seeds=None, temperature=1e-3, opening_temperature=1.0,
-                 opening_plies=30, openings=None, max_plies=None, arena_words=1 << 20):
+                 opening_plies=30, openings=None, max_plies=None, arena_words=1 << 20, rules="reference"):
+        """rules: 'reference' or 'strict' (every engine searches strictly legal moves only; a side without one is mated and loses;
+        needs search_threads = 1; openings should then come from random_openings(..., rules='strict')).  Under strict rules a game
+        whose opening leaves the side to move without a strictly legal move is over before its first ply, won by the other side."""
         if n_games <= 0 or n_games % 2:
             raise ValueError("n_games must be a positive even number (colour-swapped pairs), got %r" % (n_games,))
-        rules._init_tables()
+        self.rules = check_rules(rules, search_threads)
+        _rules._init_tables()
         self.n, self.half = int(n_games), int(n_games) // 2
         self.temperature, self.opening_temperature, self.opening_plies = temperature, opening_temperature, int(opening_plies)
         self.max_plies = max_plies
         h = self.half
         # players[k]: half k // 2, candidate for even k; the candidate is red ('w') in the first half and black in the second
-        self.players = [_Player(candidate, h, playouts, search_threads, arena_words, 0, 0),
-                        _Player(best, h, playouts, search_threads, arena_words, 1, 0),
-                        _Player(candidate, h, playouts, search_threads, arena_words, 1, h),
-                        _Player(best, h, playouts, search_threads, arena_words, 0, h)]
+        self.players = [_Player(candidate, h, playouts, search_threads, arena_words, 0, 0, self.rules),
+                        _Player(best, h, playouts, search_threads, arena_words, 1, 0, self.rules),
+                        _Player(candidate, h, playouts, search_threads, arena_words, 1, h, self.rules),
+                        _Player(best, h, playouts, search_threads, arena_words, 0, h, self.rules)]
         seeds = range(self.n) if seeds is None else seeds
         self._mt = np.zeros((self.n, MT_WORDS), dtype=np.uint32)
         for g, sd in enumerate(seeds):
             st = np.random.RandomState(int(sd)).get_state()
             self._mt[g, :624], self._mt[g, 624] = st[1], st[2]
         if openings is None:
-            ob = rules.state_to_board(rules.START_STATE)[None]
+            ob = _rules.state_to_board(_rules.START_STATE)[None]
             os_, orr = np.zeros(1, np.uint8), np.zeros(1, np.int32)
         else:
             ob, os_, orr = (np.asarray(a) for a in openings)
@@ -175,6 +190,11 @@ class Match:
         self.winner = np.full(self.n, -1, dtype=np.int64)              # 0 'w', 1 'b', 2 draw
         self.adjudicated = np.zeros(self.n, dtype=bool)
         self.ply = 0
+        if self.rules == "strict":            # an opening whose side to move has no strictly legal move: reset marked it mated
+            st = self.players[0].engine.status()
+            over = np.tile(st["terminal"] == TERM_MATED, 2)
+            self.winner[over] = np.tile(st["winner"].astype(np.int64), 2)[over]
+            self.live[over] = False
 
     def _to_move(self, p):
         return self.live[p.lo:p.hi] & (self.sides[p.lo:p.hi] == p.colour)
@@ -228,7 +248,8 @@ class Match:
             self.sides[lo:hi] = a["side"]
             term = live[lo:hi] & (a["terminal"] != 0)
             gi = lo + np.nonzero(term)[0]
-            self.winner[gi] = np.where(a["terminal"][term] == 1, a["winner"][term], 2)
+            won = (a["terminal"][term] == 1) | (a["terminal"][term] == TERM_MATED)           # a king taken, or mated (strict rules)
+            self.winner[gi] = np.where(won, a["winner"][term], 2)
             self.live[gi] = False
         for p in self.players:
             p.engine.raise_on_error()
@@ -262,7 +283,7 @@ class Match:
             res = "running" if w < 0 else "draw" if w == 2 else ("win" if w == cc else "loss")
             games.append(dict(game=g, pair=g % self.half, opening=int(self.opening[g]), candidate_colour="wb"[cc], result=res,
                               winner="?" if w < 0 else "wbt"[w], plies=int(self.plies[g]), adjudicated=bool(self.adjudicated[g]),
-                              moves=list(self.moves[g]), labels=[rules.move_to_label(m) for m in self.moves[g]]))
+                              moves=list(self.moves[g]), labels=[_rules.move_to_label(m) for m in self.moves[g]]))
         return MatchResult(games)
 
     def run(self):
@@ -289,7 +310,9 @@ def main(argv=None):
     ap.add_argument("--best_seed", type=int, default=0, help="seed of a freshly initialised best network (no --best)")
     ap.add_argument("--games", type=int, default=400)
     ap.add_argument("--playouts", type=int, default=400)
-    ap.add_argument("--search_threads", type=int, default=16)
+    ap.add_argument("--search_threads", type=int, default=None, help="default 16 (reference rules) or 1 (strict rules)")
+    ap.add_argument("--rules", choices=("reference", "strict"), default="reference",
+                    help="strict: both players search strictly legal moves only and a side without one is mated")
     ap.add_argument("--res_block_nums", type=int, default=7)
     ap.add_argument("--precision", default="fp16")
     ap.add_argument("--threshold", type=float, default=0.55)
@@ -304,10 +327,11 @@ def main(argv=None):
     a = ap.parse_args(argv)
     cand = _network(a.candidate, a.candidate_seed, a.res_block_nums, a.precision)
     best = _network(a.best, a.best_seed, a.res_block_nums, a.precision)
-    openings = random_openings(a.openings, a.opening_moves, a.seed) if a.openings > 0 else None
-    m = Match(cand, best, a.games, a.playouts, search_threads=a.search_threads, seeds=[a.seed + g for g in range(a.games)],
+    threads = a.search_threads if a.search_threads is not None else (1 if a.rules == "strict" else 16)
+    openings = random_openings(a.openings, a.opening_moves, a.seed, rules=a.rules) if a.openings > 0 else None
+    m = Match(cand, best, a.games, a.playouts, search_threads=threads, seeds=[a.seed + g for g in range(a.games)],
               temperature=a.temperature, opening_temperature=a.opening_temperature, opening_plies=a.opening_plies, openings=openings,
-              max_plies=a.max_plies)
+              max_plies=a.max_plies, rules=a.rules)
     r = m.run()
     if a.json:
         with open(a.json, "w") as f:

@@ -56,7 +56,7 @@ enum { H_FLAGS = 0, H_DONE, H_TARGET, H_RR, H_ROOTN, H_ROOTCNT, H_ROOTBASE, H_AL
 #define F_SETPEND(f, p) (((f) & ~6u) | ((uint32_t)(p) << 1))
 #define F_SIDE 8u
 #define F_CUR 16u
-#define F_TERM(f) (((f) >> 8) & 3u)                 // 0 running, 1 king captured, 2 draw
+#define F_TERM(f) (((f) >> 8) & 3u)                 // 0 running, 1 king captured, 2 draw, 3 mated (strict engines)
 #define F_WIN(f) ((int)(((f) >> 10) & 3u) - 1)      // -1 none, 0 'w', 1 'b'
 
 namespace {
@@ -237,6 +237,54 @@ __device__ int expand_reserve(const Dev &E, WarpSmem &S, uint32_t &alloc, uint32
     alloc = base + size;
     return n;
 }
+// Strict rules (k_wave<T, true>): parts 0 and 1 over the strictly legal moves.  warp_strict_moves' list is compacted onto
+// S.moves in move-generation order (ballot + popcount of the legal mask), then labelled as warp_leaf_moves does.  Zero strictly
+// legal moves is a mated position, not an error: the reservation is then the bare 8-word header.  Returns n >= 0, or -1 when the
+// arena is full.
+__device__ int warp_leaf_moves_strict(const Dev &E, WarpSmem &S, uint32_t &errf, int lane) {
+    const int lside = S.board[90];
+    uint32_t legal[4];
+    int fl;
+    int n = cz::warp_strict_moves(S.board, lside, S.moves, S.scratch, lane, legal, fl);
+    if (n > CZ_MAXCHILD) { errf |= CZ_ERR_CHILDREN; n = CZ_MAXCHILD; }
+    uint16_t mv[4];
+#pragma unroll
+    for (int k = 0; k < 4; k++) { const int i = lane + 32 * k; mv[k] = i < n ? S.moves[i] : (uint16_t)0; }
+    __syncwarp();
+    const uint32_t below = (1u << lane) - 1u;
+    int m = 0;
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+        if ((legal[k] >> lane) & 1u) S.moves[m + __popc(legal[k] & below)] = mv[k];
+        m += __popc(legal[k]);
+    }
+    __syncwarp();
+    for (int i = lane; i < m; i += 32) {
+        const int v = S.moves[i];
+        int src = v & 127, dst = v >> 7;
+        if (lside == 1) {
+            src = (9 - src / 9) * 9 + src % 9;
+            dst = (9 - dst / 9) * 9 + dst % 9;
+        }
+        int li = __ldg(E.label_of + src * CZ_NSQ + dst);
+        if (li < 0) { errf |= CZ_ERR_NOLABEL; li = 0; }
+        S.li[i] = (uint16_t)li;
+    }
+    __syncwarp();
+    return m;
+}
+__device__ int expand_reserve_strict(const Dev &E, WarpSmem &S, uint32_t &alloc, uint32_t &base, uint32_t &errf, int lane) {
+    uint32_t ef = 0;
+    const int n = warp_leaf_moves_strict(E, S, ef, lane);
+    const uint32_t cs = (uint32_t)((n + 7) & ~7), size = HDR + (uint32_t)E.narr * cs;
+    base = alloc;
+    if ((long long)base + size > E.A) ef |= CZ_ERR_ARENA;
+    ef = __reduce_or_sync(CZ_FULL, ef);
+    errf |= ef;
+    if (ef & CZ_ERR_ARENA) return -1;
+    alloc = base + size;
+    return n;
+}
 // 2: prior gather (lg = this leaf's logits row), serial float32 normalisation, block write
 __device__ void expand_write(uint32_t *ar, WarpSmem &S, const float *lg, int n, uint32_t base, int lane, bool with_q = false) {
     for (int i = lane; i < n; i += 32) S.ps[i] = __ldg(lg + S.li[i]);
@@ -367,7 +415,11 @@ __device__ __forceinline__ uint32_t select_child(const BlockRegs &R, int cnt, in
 // One wave for one game (one warp): consume the previous evaluation, then run playouts until the next leaf.
 // Launch shape: one CTA per SM whenever the games fit (warps per CTA = ceil(B / #SMs), <= MAX_WPB), so that every SM carries
 // the same number of game-warps; shared memory is sized per launch (sizeof(WarpSmem) per warp).
-template <typename T>
+// STRICT (engines created with CZ_RULES_STRICT): a node's children are its strictly legal moves; a node with none is mated.  Its
+// block is the bare 8-word header (count 0, linked under its edge with n_grandchildren 0); the playout that expanded it backs up
+// as if the network had returned -1 for the side to move there, and a later descent onto it is a terminal worth +1 to the edge.
+// A game whose root is mated leaves the search.
+template <typename T, bool STRICT>
 __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave(Dev E, T *nn_in, const float *logits, const float *value) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     WarpSmem *smem = reinterpret_cast<WarpSmem *>(smem_raw);
@@ -407,11 +459,15 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave(Dev E, T *nn_in, const
         if (lane < 24) reinterpret_cast<uint32_t *>(S.board)[lane] = lbw;
         __syncwarp();
         uint32_t base;
-        const int n = expand_reserve(E, S, alloc, base, errf, lane);
-        const bool ok = n > 0;
+        int n;
+        if constexpr (STRICT) n = expand_reserve_strict(E, S, alloc, base, errf, lane);
+        else n = expand_reserve(E, S, alloc, base, errf, lane);
+        const bool ok = STRICT ? n >= 0 : n > 0;
         if (pend == 1) {
             // leaf returns -v (main.py:384); on an engine error the playout is closed with 0
-            const float v = ok ? -val : 0.0f;
+            float v = ok ? -val : 0.0f;
+            if constexpr (STRICT) { if (n == 0) v = 1.0f; }          // mated leaf: the network's value is replaced by -1
+
             if (lane < depth && lane < SPATH) backup_edge(ar, pth, lane, depth, v, bW, bN, false);
             for (int d = SPATH + lane; d < depth; d += 32) {          // (paths longer than the prefetch window)
                 const uint2 pe = E.path[(size_t)g * MAXD + d];
@@ -453,7 +509,8 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave(Dev E, T *nn_in, const
     }
 
     uint32_t maxdep = HGET(H_MAXDEPTH);
-    if (!pend) {
+    if constexpr (STRICT) { if (!pend && root_cnt == 0) flags &= ~F_ACTIVE; }     // mated root: nothing to search
+    if (!pend && !(STRICT && root_cnt == 0)) {
         const int side0 = (flags & F_SIDE) ? 1 : 0, rr0 = (int)HGET(H_RR);
         unsigned long long rhash = 0;
         if (E.hash_on) rhash = (unsigned long long)HGET(H_HASHLO) | ((unsigned long long)HGET(H_HASHHI) << 32);
@@ -521,6 +578,9 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave(Dev E, T *nn_in, const
                         break;
                     }
                     if (rr >= 60) { tval = 0.0f; break; }        // main.py:415-416
+                    if constexpr (STRICT) {                      // expanded without children: the side to move is mated
+                        if (child != NONE && ((meta >> 16) & 0xFFu) == 0) { tval = 1.0f; break; }
+                    }
                     if (child == NONE) { leaf = true; break; }   // main.py:357: not expanded -> evaluate
                     base = child;
                     cnt = (int)((meta >> 16) & 0xFFu);
@@ -1267,6 +1327,9 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) k_play(Dev E) {
 // that carries the move exactly as k_play does; an unexpanded root (fresh reset, or re-rooted onto an unvisited child) checks the
 // move against the position's legal moves and moves on to an empty tree at the new position (no search is run for it, unlike
 // human_move).  A move that is not legal there, or any move in a finished game, sets CZ_ERR_ILLEGAL and leaves the game as it was.
+// STRICT: an unexpanded root accepts only a strictly legal move (an expanded root's children are strictly legal already), among the
+// first 128 pseudo-legal moves -- the moves an expansion keeps (more is CZ_ERR_CHILDREN, reachable on set-up boards only).
+template <bool STRICT>
 __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) k_play_moves(Dev E, const uint16_t *moves) {
     __shared__ WarpSmem smem[WARPS_PER_BLOCK];
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, g = blockIdx.x * WARPS_PER_BLOCK + w;
@@ -1289,10 +1352,21 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) k_play_moves(Dev E, cons
             WarpSmem &S = smem[w];
             for (int i = lane; i < 90; i += 32) S.board[i] = b[i];
             __syncwarp();
-            int n = cz::warp_legal_moves(S.board, (flags & F_SIDE) ? 1 : 0, S.moves, S.scratch, lane);
-            if (n > 136) n = 136;
             bool hit = false;
-            for (int i = lane; i < n; i += 32) hit |= S.moves[i] == mv;
+            if constexpr (STRICT) {
+                uint32_t legal[4];
+                int fl;
+                const int n = cz::warp_strict_moves(S.board, (flags & F_SIDE) ? 1 : 0, S.moves, S.scratch, lane, legal, fl);
+#pragma unroll
+                for (int k = 0; k < 4; k++) {
+                    const int i = lane + 32 * k;
+                    hit |= i < n && ((legal[k] >> lane) & 1u) && S.moves[i] == mv;
+                }
+            } else {
+                int n = cz::warp_legal_moves(S.board, (flags & F_SIDE) ? 1 : 0, S.moves, S.scratch, lane);
+                if (n > 136) n = 136;
+                for (int i = lane; i < n; i += 32) hit |= S.moves[i] == mv;
+            }
             if (__any_sync(CZ_FULL, hit)) {
                 const int src = mv & 127, dst = (mv >> 7) & 127;
                 if (lane == 0) {
@@ -1307,6 +1381,40 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) k_play_moves(Dev E, cons
     }
     if (lane == 0) atomicOr(h + H_ERR, CZ_ERR_ILLEGAL);
     write_status(E, g, h, b, 0.0f, lane);
+}
+
+// ---- strict engines: a root without a strictly legal move ends the game ----------------------------------------------------
+// After every change of a root (reset, set_root_meta, play, play_moves) of a strict engine: a running game (mask[g], NULL = all)
+// whose side to move has no strictly legal move -- checkmate or stalemate -- gets terminal code 3 and the side that just moved as
+// the winner, in its header line and in its packed status record.  An expanded root is mated iff it has no children (they are
+// strictly legal); an unexpanded one runs cz::warp_strict_moves on the root board.
+__global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) k_root_mate(Dev E, const uint8_t *mask) {
+    __shared__ WarpSmem smem[WARPS_PER_BLOCK];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, g = blockIdx.x * WARPS_PER_BLOCK + w;
+    if (g >= E.B || (mask && !mask[g])) return;
+    uint32_t *h = E.hdr + (size_t)g * HW;
+    const uint32_t flags = h[H_FLAGS];
+    const int rcnt = (int)h[H_ROOTCNT];
+    if (F_TERM(flags) != 0 || rcnt > 0) return;
+    const int side = (flags & F_SIDE) ? 1 : 0;
+    bool mated = rcnt == 0;
+    if (!mated) {
+        WarpSmem &S = smem[w];
+        const uint8_t *b = E.root_board + (size_t)g * 96;
+        for (int i = lane; i < 90; i += 32) S.board[i] = b[i];
+        __syncwarp();
+        uint32_t legal[4];
+        int fl;
+        cz::warp_strict_moves(S.board, side, S.moves, S.scratch, lane, legal, fl);
+        mated = (fl & 2) != 0;
+    }
+    __syncwarp();
+    if (mated && lane == 0) {
+        h[H_FLAGS] = (flags & ~(F_ACTIVE | 0xF00u)) | (3u << 8) | ((uint32_t)(side ^ 1) + 1u) << 10;
+        uint8_t *o = E.st_status + (size_t)g * CZ_STATUS_BYTES;
+        o[91] = 3;
+        o[92] = (uint8_t)(side ^ 1);
+    }
 }
 
 // ---- stateless batched rules ------------------------------------------------------------
@@ -1409,7 +1517,8 @@ __global__ void k_apply(uint8_t *boards, const uint16_t *moves, int n, uint8_t *
 // 16 bytes), then per game: hdr [16] | root board [24] | counters 5 x u64 [10] | pad [2] | fifo [FW] (FIFO engines) | arena [alloc].
 // Every section is a multiple of 4 words at a 16-byte aligned offset, so both directions copy with copy_block.
 #define SNAP_MAGIC 0x485350414E535A43ull   // "CZSNAPSH"
-#define SNAP_FORMAT 1u
+#define SNAP_FORMAT 1u                     // reference-rules engines
+#define SNAP_FORMAT_STRICT 2u              // strict-rules engines: the same layout; count-0 blocks and terminal code 3 may occur
 #define SNAP_HEAD_WORDS 12                 // magic | format, cz_version | zobrist checksum | B, K | narr, fixed words | reserved
 enum { S_HDR = 0, S_BOARD = 16, S_CNT = 40, S_FIFO = 52 };
 
@@ -1513,6 +1622,7 @@ struct cz_engine {
     int32_t *d_rr = nullptr;
     uint32_t *d_snap = nullptr;      // device staging of snapshot blobs, grown on demand
     size_t snap_cap = 0;
+    int rules = CZ_RULES_REFERENCE;  // CZ_RULES_STRICT: k_wave<T, true>, k_play_moves<true> and k_root_mate after every root change
 };
 
 extern "C" {
@@ -1771,6 +1881,13 @@ int cz_engine_create_fifo(int n_games, int64_t arena_words, int device, int sear
     return create_engine(n_games, arena_words, device, search_threads, true, out);
 }
 int cz_engine_is_fifo(const cz_engine *e) { return e ? (e->d.fifo != nullptr) : CZ_EINVAL; }
+int cz_engine_create_rules(int n_games, int64_t arena_words, int device, int rules, cz_engine **out) {
+    if (rules != CZ_RULES_REFERENCE && rules != CZ_RULES_STRICT) return fail(CZ_EINVAL, "cz_engine_create_rules: rules must be CZ_RULES_REFERENCE or CZ_RULES_STRICT");
+    const int rc = create_engine(n_games, arena_words, device, 1, false, out);
+    if (rc == CZ_OK) (*out)->rules = rules;
+    return rc;
+}
+int cz_engine_rules(const cz_engine *e) { return e ? e->rules : CZ_EINVAL; }
 
 extern "C++" {
 static int create_engine(int n_games, int64_t arena_words, int device, int leaves, bool fifo, cz_engine **out) {
@@ -1845,6 +1962,16 @@ int cz_engine_destroy(cz_engine *e) {
 
 int cz_engine_n_games(const cz_engine *e) { return e ? e->d.B : CZ_EINVAL; }
 
+extern "C++" {
+// strict engines only: k_root_mate after a kernel that changed roots (same stream; mask: device copy or NULL)
+static int root_mate(cz_engine *e, cudaStream_t st, const uint8_t *dmask) {
+    if (e->rules != CZ_RULES_STRICT) return CZ_OK;
+    k_root_mate<<<nblk(e->d.B, WARPS_PER_BLOCK), 32 * WARPS_PER_BLOCK, 0, st>>>(e->d, dmask);
+    CUDA_TRY(cudaGetLastError());
+    return CZ_OK;
+}
+}  // extern "C++"
+
 int cz_engine_reset(cz_engine *e, void *stream, const uint8_t *mask, const uint8_t *boards, const uint8_t *sides, const int32_t *rr) {
     if (!e) return fail(CZ_EINVAL, "null engine");
     cudaStream_t st = (cudaStream_t)stream;
@@ -1857,6 +1984,8 @@ int cz_engine_reset(cz_engine *e, void *stream, const uint8_t *mask, const uint8
     k_reset<<<nblk(e->d.B, 128), 128, 0, st>>>(e->d, mask ? e->d_mask : nullptr, boards ? e->d_boards : nullptr,
                                                sides ? e->d_sides : nullptr, rr ? e->d_rr : nullptr);
     CUDA_TRY(cudaGetLastError());
+    const int rc = root_mate(e, st, mask ? e->d_mask : nullptr);
+    if (rc) return rc;
     CUDA_TRY(cudaStreamSynchronize(st));   // host buffers may be pageable: do not return before they are consumed
     return CZ_OK;
 }
@@ -1871,6 +2000,8 @@ int cz_engine_set_root_meta(cz_engine *e, void *stream, const uint8_t *mask, con
     if (rr) CUDA_TRY(cudaMemcpyAsync(e->d_rr, rr, B * 4, cudaMemcpyHostToDevice, st));
     k_set_meta<<<nblk(e->d.B, 128), 128, 0, st>>>(e->d, mask ? e->d_mask : nullptr, sides ? e->d_sides : nullptr, rr ? e->d_rr : nullptr);
     CUDA_TRY(cudaGetLastError());
+    const int rc = root_mate(e, st, mask ? e->d_mask : nullptr);
+    if (rc) return rc;
     CUDA_TRY(cudaStreamSynchronize(st));
     return CZ_OK;
 }
@@ -1909,10 +2040,19 @@ int cz_engine_wave(cz_engine *e, void *stream, void *nn_in, int nn_dtype, const 
         CUDA_TRY(cudaGetLastError());
         return CZ_OK;
     }
-    if (nn_dtype == CZ_F32) k_wave<float><<<gr, bl, sm, st>>>(e->d, (float *)nn_in, logits, value);
-    else if (nn_dtype == CZ_BF16) k_wave<__nv_bfloat16><<<gr, bl, sm, st>>>(e->d, (__nv_bfloat16 *)nn_in, logits, value);
-    else if (nn_dtype == CZ_F16) k_wave<__half><<<gr, bl, sm, st>>>(e->d, (__half *)nn_in, logits, value);
-    else if (nn_dtype == CZ_BOARD) k_wave<uint8_t><<<gr, bl, sm, st>>>(e->d, (uint8_t *)nn_in, logits, value);
+    if (e->rules == CZ_RULES_STRICT) {
+        if (nn_dtype == CZ_F32) k_wave<float, true><<<gr, bl, sm, st>>>(e->d, (float *)nn_in, logits, value);
+        else if (nn_dtype == CZ_BF16) k_wave<__nv_bfloat16, true><<<gr, bl, sm, st>>>(e->d, (__nv_bfloat16 *)nn_in, logits, value);
+        else if (nn_dtype == CZ_F16) k_wave<__half, true><<<gr, bl, sm, st>>>(e->d, (__half *)nn_in, logits, value);
+        else if (nn_dtype == CZ_BOARD) k_wave<uint8_t, true><<<gr, bl, sm, st>>>(e->d, (uint8_t *)nn_in, logits, value);
+        else return fail(CZ_EINVAL, "wave: nn_dtype");
+        CUDA_TRY(cudaGetLastError());
+        return CZ_OK;
+    }
+    if (nn_dtype == CZ_F32) k_wave<float, false><<<gr, bl, sm, st>>>(e->d, (float *)nn_in, logits, value);
+    else if (nn_dtype == CZ_BF16) k_wave<__nv_bfloat16, false><<<gr, bl, sm, st>>>(e->d, (__nv_bfloat16 *)nn_in, logits, value);
+    else if (nn_dtype == CZ_F16) k_wave<__half, false><<<gr, bl, sm, st>>>(e->d, (__half *)nn_in, logits, value);
+    else if (nn_dtype == CZ_BOARD) k_wave<uint8_t, false><<<gr, bl, sm, st>>>(e->d, (uint8_t *)nn_in, logits, value);
     else return fail(CZ_EINVAL, "wave: nn_dtype");
     CUDA_TRY(cudaGetLastError());
     return CZ_OK;
@@ -2012,6 +2152,8 @@ int cz_engine_play_status(cz_engine *e, void *stream, const int32_t *child_index
     CUDA_TRY(cudaMemcpyAsync(e->d.st_choice, e->h_choice, B * 4, cudaMemcpyHostToDevice, st));
     k_play<<<nblk(e->d.B, WARPS_PER_BLOCK), 32 * WARPS_PER_BLOCK, 0, st>>>(e->d);
     CUDA_TRY(cudaGetLastError());
+    const int rc = root_mate(e, st, nullptr);
+    if (rc) return rc;
     if (status) CUDA_TRY(cudaMemcpyAsync(e->h_status, e->d.st_status, B * CZ_STATUS_BYTES, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));   // h_choice is reused by the next call
     if (status) memcpy(status, e->h_status, B * CZ_STATUS_BYTES);
@@ -2029,8 +2171,11 @@ int cz_engine_play_moves(cz_engine *e, void *stream, const uint16_t *moves, uint
     uint16_t *dm = reinterpret_cast<uint16_t *>(e->d.st_choice);
     memcpy(hm, moves, B * 2);
     CUDA_TRY(cudaMemcpyAsync(dm, hm, B * 2, cudaMemcpyHostToDevice, st));
-    k_play_moves<<<nblk(e->d.B, WARPS_PER_BLOCK), 32 * WARPS_PER_BLOCK, 0, st>>>(e->d, dm);
+    if (e->rules == CZ_RULES_STRICT) k_play_moves<true><<<nblk(e->d.B, WARPS_PER_BLOCK), 32 * WARPS_PER_BLOCK, 0, st>>>(e->d, dm);
+    else k_play_moves<false><<<nblk(e->d.B, WARPS_PER_BLOCK), 32 * WARPS_PER_BLOCK, 0, st>>>(e->d, dm);
     CUDA_TRY(cudaGetLastError());
+    const int rc = root_mate(e, st, nullptr);
+    if (rc) return rc;
     if (status) CUDA_TRY(cudaMemcpyAsync(e->h_status, e->d.st_status, B * CZ_STATUS_BYTES, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));   // h_choice is reused by the next call
     if (status) memcpy(status, e->h_status, B * CZ_STATUS_BYTES);
@@ -2141,7 +2286,8 @@ int cz_engine_tree_signature(cz_engine *e, void *stream, int game, int64_t *out,
         if (e->d.narr == 6) memcpy(&Q, &blk[5 * cs + i], 4);     // FIFO mode: the stored Q of the last back_up_value
         uint32_t qb;
         memcpy(&qb, &Q, 4);
-        const int nch = child != NONE ? (int)((meta >> 16) & 0xFFu) : 0;
+        int nch = child != NONE ? (int)((meta >> 16) & 0xFFu) : 0;
+        if (child != NONE && nch == 0) nch = -1;                 // expanded without children: a mated node (strict engines)
         if (k < cap && out) {
             int64_t *r = out + 6 * k;
             r[0] = L.of[(meta & 127) * CZ_NSQ + ((meta >> 7) & 127)];
@@ -2179,9 +2325,12 @@ static int snap_fail(long long g, const char *what) {
 }
 // Every block reachable from the root of one game section (ar = its arena words [0, alloc)); nullptr or the failed check.  Blocks
 // reached must be disjoint (so play_child's compaction copies at most alloc words) and children lie above their parent (no cycle).
-static const char *check_tree(const uint32_t *ar, uint32_t alloc, uint32_t rbase, int rcnt, int narr) {
-    if (rcnt <= 0) return nullptr;
+// strict (format 2): a mated node -- an expanded child with n_grandchildren 0, or a root with count 0 -- is a bare 8-word block,
+// so the words right after it are the end of the tree or the start of another reachable block.
+static const char *check_tree(const uint32_t *ar, uint32_t alloc, uint32_t rbase, int rcnt, int narr, bool strict) {
+    if (rcnt < 0 || (rcnt == 0 && !strict)) return nullptr;
     std::vector<uint8_t> used(alloc / 8 + 1, 0);        // 8-word granules covered by a reachable block
+    std::vector<uint32_t> mated;                         // bases of the count-0 blocks
     struct Fr { uint32_t base; int cnt; };
     std::vector<Fr> st{{rbase, rcnt}};
     while (!st.empty()) {
@@ -2195,6 +2344,7 @@ static const char *check_tree(const uint32_t *ar, uint32_t alloc, uint32_t rbase
             if (used[k]) return "blocks overlap or a block is reached twice";
             used[k] = 1;
         }
+        if (f.cnt == 0) mated.push_back(f.base);
         const uint32_t *blk = ar + f.base + HDR;
         for (int i = 0; i < f.cnt; i++) {
             const uint32_t meta = blk[3 * cs + i], child = blk[4 * cs + i];
@@ -2205,11 +2355,13 @@ static const char *check_tree(const uint32_t *ar, uint32_t alloc, uint32_t rbase
                 if (ngc) return "META n_grandchildren set on an unexpanded child";
                 continue;
             }
-            if (ngc == 0) return "expanded child with META n_grandchildren 0";
+            if (ngc == 0 && !strict) return "expanded child with META n_grandchildren 0";
             if (child <= f.base) return "child pointer not above its parent's base";
             st.push_back({child, ngc});
         }
     }
+    for (uint32_t b : mated)
+        if (b + HDR != alloc && !used[(b + HDR) / 8]) return "count-0 block longer than its 8-word header (words after it belong to no block)";
     return nullptr;
 }
 // Section offsets of every game from the header lines (one device->host copy); refuses a game that is not at rest.
@@ -2244,12 +2396,22 @@ static int snapshot_staging(cz_engine *e, size_t bytes) {
 }  // extern "C++"
 
 int cz_snapshot_check(const void *in, int64_t bytes, int n_games, int leaves, int narr, int64_t arena_words) {
+    return cz_snapshot_check_rules(in, bytes, n_games, leaves, narr, arena_words, CZ_RULES_REFERENCE);
+}
+
+int cz_snapshot_check_rules(const void *in, int64_t bytes, int n_games, int leaves, int narr, int64_t arena_words, int rules) {
+    if (rules != CZ_RULES_REFERENCE && rules != CZ_RULES_STRICT) return snap_fail(-1, "bad rules argument");
     if (n_games <= 0 || leaves <= 0 || (narr != 5 && narr != 6) || arena_words <= 0) return snap_fail(-1, "bad engine arguments");
     if (!in || bytes < 48) return snap_fail(-1, "truncated blob: shorter than its head");
     if ((uintptr_t)in & 7) return snap_fail(-1, "blob not 8-byte aligned");
     const uint64_t *head = (const uint64_t *)in;
     if (head[0] != SNAP_MAGIC) return snap_fail(-1, "bad magic: not an engine snapshot");
-    if ((uint32_t)head[1] != SNAP_FORMAT) return snap_fail(-1, "unsupported format version");
+    const uint32_t format = (uint32_t)head[1];
+    const bool strict = rules == CZ_RULES_STRICT;
+    if (format == (strict ? SNAP_FORMAT : SNAP_FORMAT_STRICT))
+        return snap_fail(-1, strict ? "unsupported format version for a strict-rules engine: rules differ (format 1 holds reference-rules games)"
+                                    : "unsupported format version for a reference-rules engine: rules differ (format 2 holds strict-rules games)");
+    if (format != (strict ? SNAP_FORMAT_STRICT : SNAP_FORMAT)) return snap_fail(-1, "unsupported format version");
     if (head[2] != zobrist_checksum()) return snap_fail(-1, "Zobrist table checksum differs from this library's");
     const int B = (int32_t)(uint32_t)head[3], K = (int32_t)(uint32_t)(head[3] >> 32), na = (int32_t)(uint32_t)head[4];
     const uint32_t fixed = (uint32_t)(head[4] >> 32);
@@ -2274,7 +2436,8 @@ int cz_snapshot_check(const void *in, int64_t bytes, int n_games, int leaves, in
         if (!header_at_rest(h)) return snap_fail(g, "not at rest: an expansion is pending or playouts are owed");
         if (f & ~0xF1Fu) return snap_fail(g, "unknown flag bits");
         const uint32_t term = F_TERM(f), win = (f >> 10) & 3u;
-        if (term == 3 || win == 3 || (term == 1) != (win != 0)) return snap_fail(g, "bad terminal / winner code");
+        if (term == 3 && !strict) return snap_fail(g, "terminal code 3 (mated) in a format 1 (reference rules) blob");
+        if (win == 3 || (term == 1 || term == 3) != (win != 0)) return snap_fail(g, "bad terminal / winner code");
         const int rcnt = (int)h[H_ROOTCNT];
         if (rcnt < -1 || rcnt > CZ_MAXCHILD) return snap_fail(g, "root child count outside {-1, 0..128}");
         const uint8_t *b = (const uint8_t *)(s + S_BOARD);
@@ -2282,7 +2445,7 @@ int cz_snapshot_check(const void *in, int64_t bytes, int n_games, int leaves, in
             if (b[i] > (i < CZ_NSQ ? 14 : 0)) return snap_fail(g, "root board piece code outside 0..14 (or padding not zero)");
         if (narr == 6 && (s[S_FIFO + FI_ITER] || s[S_FIFO + FI_NCUR] || s[S_FIFO + FI_NQ]))
             return snap_fail(g, "FIFO event loop not at rest");
-        const char *why = check_tree(s + fixed, alloc, h[H_ROOTBASE], rcnt, narr);
+        const char *why = check_tree(s + fixed, alloc, h[H_ROOTBASE], rcnt, narr, strict);
         if (why) return snap_fail(g, why);
     }
     return CZ_OK;
@@ -2308,7 +2471,7 @@ int cz_engine_snapshot(cz_engine *e, void *stream, void *out, int64_t cap, int64
     if (cap < total) return fail(CZ_EINVAL, "cz_engine_snapshot: cap is smaller than the snapshot (see cz_engine_snapshot_size)");
     std::vector<uint64_t> head((size_t)hw / 2, 0ull);
     head[0] = SNAP_MAGIC;
-    head[1] = SNAP_FORMAT | ((uint64_t)(uint32_t)cz_version() << 32);
+    head[1] = (e->rules == CZ_RULES_STRICT ? SNAP_FORMAT_STRICT : SNAP_FORMAT) | ((uint64_t)(uint32_t)cz_version() << 32);
     head[2] = zobrist_checksum();
     head[3] = (uint32_t)B | ((uint64_t)(uint32_t)e->d.K << 32);
     head[4] = (uint32_t)e->d.narr | ((uint64_t)snap_fixed_words(e->d.narr) << 32);
@@ -2326,7 +2489,7 @@ int cz_engine_snapshot(cz_engine *e, void *stream, void *out, int64_t cap, int64
 
 int cz_engine_restore(cz_engine *e, void *stream, const void *in, int64_t bytes) {
     if (!e) return fail(CZ_EINVAL, "cz_engine_restore: null engine");
-    int rc = cz_snapshot_check(in, bytes, e->d.B, e->d.K, e->d.narr, e->d.A);   // nothing on the device is written before this
+    int rc = cz_snapshot_check_rules(in, bytes, e->d.B, e->d.K, e->d.narr, e->d.A, e->rules);   // nothing on the device is written before this
     if (rc) return rc;
     CUDA_TRY(cudaSetDevice(e->device));
     rc = snapshot_staging(e, (size_t)bytes);

@@ -8,7 +8,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import BF16, BOARD, F16, F32, MAXCHILD, STATUS_BYTES, EngineError, check, lib
+from ._lib import BF16, BOARD, F16, F32, MAXCHILD, RULES, STATUS_BYTES, EngineError, check, lib
 
 _DT = {torch.float32: F32, torch.bfloat16: BF16, torch.float16: F16, torch.uint8: BOARD}
 
@@ -21,14 +21,33 @@ def _stream():
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
+def check_rules(rules, search_threads=1, leaves=1):
+    """The engine rules `rules` names ('reference' or 'strict'); ValueError for another name, and for strict rules with more than one
+    leaf per game and wave (leaf-parallel or search_threads > 1 engines play by the reference rules only).  search_threads as SelfPlay,
+    Match and Trainer take it: 1 (or None) is the one-leaf engine."""
+    if rules not in RULES:
+        raise ValueError("rules must be 'reference' or 'strict', not %r" % (rules,))
+    if rules == "strict" and (int(search_threads or 1) != 1 or int(leaves) != 1):
+        raise ValueError("strict rules need the one-leaf engine (search_threads = 1, leaves = 1)")
+    return rules
+
+
 class Engine:
-    def __init__(self, n_games, arena_words=0, device=None, leaves=1, search_threads=None):
+    def __init__(self, n_games, arena_words=0, device=None, leaves=1, search_threads=None, rules="reference"):
         """leaves > 1: leaf-parallel engine (up to `leaves` leaves per game per wave; network rows = n_games*leaves).
         leaves == -1: the leaf-parallel kernel with one slot (test hook).
         search_threads = K: the reference's search_threads schedule in canonical FIFO form (bit-exact with the reference's
-        uvloop runs wherever those are reproducible); network rows = n_games*K."""
+        uvloop runs wherever those are reproducible); network rows = n_games*K.
+        rules: 'reference' (pseudo-legal moves, a game ends when a king is taken) or 'strict' (strictly legal moves only; a side
+        without one is mated, terminal code 3; cz_engine_create_rules).  Strict rules need the one-leaf engine: no search_threads
+        (any search_threads value, 1 included, builds the FIFO engine) and leaves = 1."""
+        check_rules(rules, 1, leaves)
+        if rules == "strict" and search_threads is not None:
+            raise ValueError("strict rules need the one-leaf engine: search_threads = %r builds the search_threads schedule's (FIFO) "
+                             "engine, which plays by the reference rules; leave search_threads unset" % (search_threads,))
         if not torch.cuda.is_available():
             raise EngineError("cchess_zero_b200 needs a CUDA device (no CPU fallback exists)")
+        self.rules = rules
         self.device = torch.cuda.current_device() if device is None else int(device)
         self.B = int(n_games)
         self.fifo = search_threads is not None
@@ -37,10 +56,13 @@ class Engine:
         h = C.c_void_p()
         if self.fifo:
             check(lib().cz_engine_create_fifo(self.B, int(arena_words), self.device, int(search_threads), C.byref(h)), "cz_engine_create_fifo")
+        elif rules == "strict":
+            check(lib().cz_engine_create_rules(self.B, int(arena_words), self.device, RULES[rules], C.byref(h)), "cz_engine_create_rules")
         else:
             check(lib().cz_engine_create_ex(self.B, int(arena_words), self.device, int(leaves), C.byref(h)), "cz_engine_create_ex")
         self.h = h
         self.launches = 0   # kernels of csrc/cz_engine.cu launched through this handle
+        self._mate = 1 if rules == "strict" else 0          # k_root_mate after every root change of a strict engine
         self._count = torch.zeros(1, dtype=torch.int32, device="cuda:%d" % self.device)
 
     def close(self):
@@ -60,14 +82,14 @@ class Engine:
         b = None if boards is None else np.ascontiguousarray(boards, dtype=np.uint8).reshape(self.B, 90)
         s = None if sides is None else np.ascontiguousarray(sides, dtype=np.uint8)
         r = None if rr is None else np.ascontiguousarray(rr, dtype=np.int32)
-        self.launches += 1
+        self.launches += 1 + self._mate
         check(lib().cz_engine_reset(self.h, _stream(), _hp(m), _hp(b), _hp(s), _hp(r)), "cz_engine_reset")
 
     def set_root_meta(self, sides=None, rr=None, mask=None):
         m = None if mask is None else np.ascontiguousarray(mask, dtype=np.uint8)
         s = None if sides is None else np.ascontiguousarray(sides, dtype=np.uint8)
         r = None if rr is None else np.ascontiguousarray(rr, dtype=np.int32)
-        self.launches += 1
+        self.launches += 1 + self._mate
         check(lib().cz_engine_set_root_meta(self.h, _stream(), _hp(m), _hp(s), _hp(r)), "cz_engine_set_root_meta")
 
     def begin_search(self, playouts, mask=None):
@@ -142,7 +164,7 @@ class Engine:
         from the same call: one kernel, one device->host copy, one synchronisation."""
         ci = np.ascontiguousarray(child_index, dtype=np.int32)
         assert ci.shape == (self.B,)
-        self.launches += 1
+        self.launches += 1 + self._mate
         rec = np.zeros((self.B, STATUS_BYTES), dtype=np.uint8) if want_status else None
         check(lib().cz_engine_play_status(self.h, _stream(), _hp(ci), _hp(rec)), "cz_engine_play_status")
         return self._unpack_status(rec) if want_status else None
@@ -150,10 +172,11 @@ class Engine:
     def play_moves(self, moves, want_status=True):
         """Play the given move (src | dst << 7; 0xFFFF = none) in every game, searched at the root or not: the opponent's move in a
         game where each player keeps its own tree (update_tree for a move the tree did not choose).  A move that is not legal at the
-        root, or any move in a finished game, sets the ILLEGAL error flag and leaves that game unchanged (cz_engine_play_moves)."""
+        root, or any move in a finished game, sets the ILLEGAL error flag and leaves that game unchanged (cz_engine_play_moves).  A strict
+        engine accepts only strictly legal moves."""
         mv = np.ascontiguousarray(moves, dtype=np.uint16)
         assert mv.shape == (self.B,)
-        self.launches += 1
+        self.launches += 1 + self._mate
         rec = np.zeros((self.B, STATUS_BYTES), dtype=np.uint8) if want_status else None
         check(lib().cz_engine_play_moves(self.h, _stream(), _hp(mv), _hp(rec)), "cz_engine_play_moves")
         return self._unpack_status(rec) if want_status else None
@@ -166,7 +189,8 @@ class Engine:
                     q=np.ascontiguousarray(tail[:, 2]).view(np.float32), root_N=tail[:, 3].copy())
 
     def status(self, boards=True):
-        """terminal / winner / ply / restrict_round / side / boards of every game (check_end, main.py:1380-1392)."""
+        """terminal / winner / ply / restrict_round / side / boards of every game (check_end, main.py:1380-1392).  terminal: 0 running,
+        1 king captured, 2 draw, 3 mated (strict engines; the winner is the side that just moved)."""
         rec = np.zeros((self.B, STATUS_BYTES), dtype=np.uint8)
         self.launches += 1
         check(lib().cz_engine_status_packed(self.h, _stream(), _hp(rec)), "cz_engine_status_packed")

@@ -16,9 +16,9 @@ from collections import defaultdict, deque
 import numpy as np
 import torch
 
-from . import rules
-from ._lib import MAXCHILD, MT_WORDS, NLABEL, NSQ, EngineError
-from .engine import Engine, capture_cuda_graph, run_waves
+from . import rules as _rules                        # (SelfPlay takes a `rules` argument)
+from ._lib import MAXCHILD, MT_WORDS, NLABEL, NSQ, TERM_MATED, EngineError
+from .engine import Engine, capture_cuda_graph, check_rules, run_waves
 
 
 def _flip_board(b):
@@ -35,7 +35,7 @@ def _flip_move_label_index(mv):
     s, d = int(mv) & 127, (int(mv) >> 7) & 127
     s = (9 - s // 9) * 9 + s % 9
     d = (9 - d // 9) * 9 + d % 9
-    return rules.label2i[rules.move_to_label(s | (d << 7))]
+    return _rules.label2i[_rules.move_to_label(s | (d << 7))]
 
 
 _LABEL_OF = None
@@ -149,7 +149,7 @@ class GameRecord:
         tab = _label_table()
         st, ix = [], []
         for b, side, mv in zip(self._boards, self.players, self._moves):
-            st.append(rules.board_to_state(_flip_board(b) if side == 1 else b))             # main.py:1504-1505
+            st.append(_rules.board_to_state(_flip_board(b) if side == 1 else b))             # main.py:1504-1505
             src, dst = (mv & 127).astype(np.int64), (mv >> 7).astype(np.int64)
             if side == 1:   # flipped_uci_labels for black (main.py:1507-1512): rank y -> 9-y
                 src = (9 - src // 9) * 9 + src % 9
@@ -159,7 +159,7 @@ class GameRecord:
                 raise KeyError("move outside the label table")                                # label2i[...] KeyError in the reference
             ix.append(li)
         self._states, self._pi_idx = st, ix
-        self._actions = [rules.move_to_label(mv[c]) for mv, c in zip(self._moves, self._chosen)]
+        self._actions = [_rules.move_to_label(mv[c]) for mv, c in zip(self._moves, self._chosen)]
 
     @classmethod
     def from_tuples(cls, states, pi_idx, pi_val, z):
@@ -207,11 +207,16 @@ class SelfPlay:
 
     def __init__(self, n_games, forward, playouts, seeds=None, exploration=True, temperature=1,
                  nn_dtype=torch.float32, arena_words=0, auto_reset=True, device=None, keep_records=True, plan=None,
-                 plan_factory=None, lanes=1, engine=None, hashing=False, search_threads=1, compact=None):
+                 plan_factory=None, lanes=1, engine=None, hashing=False, search_threads=1, compact=None, rules="reference"):
         """plan: an InferencePlan / NativePlan (defines the input buffer, writes logits/value in place); plan_factory(rows) builds
-        one when `plan` is not given.  lanes: 1 is the only value."""
+        one when `plan` is not given.  lanes: 1 is the only value.  rules: 'reference' or 'strict' (the search expands strictly legal
+        moves only and a side without one is mated: the game ends with terminal code 3, won by the side that moved last); strict
+        rules need search_threads = 1."""
         if lanes != 1:
             raise ValueError("SelfPlay: lanes must be 1")
+        self.rules = check_rules(rules, search_threads)
+        if engine is not None and getattr(engine, "rules", "reference") != rules:
+            raise ValueError("SelfPlay: the engine plays by the %r rules, not %r" % (getattr(engine, "rules", "reference"), rules))
         self.B = n_games
         # search_threads = K > 1: every game runs the reference's K-coroutine schedule (k_wave_fifo); the network batch has K rows per game
         self.K = max(1, int(search_threads))
@@ -221,7 +226,7 @@ class SelfPlay:
         # `engine`: an object with the Engine interface (tests drive the host loop with a CPU stand-in); the product
         # always constructs the CUDA engine here
         self.engine = engine if engine is not None else (Engine(n_games, arena_words, device, search_threads=self.K) if self.K > 1
-                                                         else Engine(n_games, arena_words, device))
+                                                         else Engine(n_games, arena_words, device, rules=rules))
         if hashing:                              # Zobrist keys of the pending leaves (must be on before a graph is captured)
             self.engine.enable_hashing(True)
         dev = torch.device("cuda", self.engine.device) if engine is None else torch.device(getattr(engine, "torch_device", "cpu"))
@@ -260,7 +265,7 @@ class SelfPlay:
         self.auto_reset = auto_reset
         self.keep_records = keep_records
         self.records = [GameRecord(g, None, temperature) for g in range(n_games)]
-        self._start_board = rules.state_to_board(rules.START_STATE)
+        self._start_board = _rules.state_to_board(_rules.START_STATE)
         self.boards = np.tile(self._start_board, (n_games, 1))
         self.sides = np.zeros(n_games, dtype=np.uint8)
         self.live = np.ones(n_games, dtype=bool)
@@ -269,7 +274,7 @@ class SelfPlay:
         self.waves = 0
         self.graph = None
         self._threads = max(1, min(16, (len(os.sched_getaffinity(0)) if hasattr(os, "sched_getaffinity") else 4)))
-        rules._init_tables()
+        _rules._init_tables()
 
     # -- evaluation step ---------------------------------------------------------------------
     def _eval(self, nn_in):
@@ -374,7 +379,7 @@ class SelfPlay:
         for g in np.nonzero(self.live & (st["terminal"] != 0))[0]:
             rec = self.records[g]
             players = np.asarray(rec.players)
-            if st["terminal"][g] == 1:                                                   # main.py:1532-1541
+            if st["terminal"][g] in (1, TERM_MATED):                                     # main.py:1532-1541; mated: strict rules
                 w = int(st["winner"][g])
                 rec.z = np.where(players == w, 1.0, -1.0)
                 rec.winner = "w" if w == 0 else "b"
@@ -533,7 +538,7 @@ class cchess_main(object):
                  num_gpus=1, res_block_nums=7, human_color="b", network=None, log_file=True, leaf_parallel=1, strict=False):
         from .mcts import MCTS_tree
         from .net import policy_value_network, policy_value_network_gpus
-        rules._init_tables()
+        _rules._init_tables()
         self.epochs = 5
         self.playout_counts = playout
         self.temperature = 1
@@ -546,7 +551,7 @@ class cchess_main(object):
         self.lr_multiplier = 1.0
         self.buffer_size = 10000
         self.data_buffer = deque(maxlen=self.buffer_size)
-        self.game_borad = rules.GameBoard()
+        self.game_borad = _rules.GameBoard()
         if network is not None:
             self.policy_value_netowrk = network
         else:  # `processor` selected CPU/GPU TensorFlow in the reference (main.py:1142); both map to the CUDA net here
@@ -564,7 +569,7 @@ class cchess_main(object):
     @staticmethod
     def flip_policy(prob):  # main.py:1152-1155
         prob = np.asarray(prob).flatten()
-        return np.asarray([prob[i] for i in rules.unflipped_index])
+        return np.asarray([prob[i] for i in _rules.unflipped_index])
 
     # ---- training (main.py:1157-1205) ------------------------------------------------------------
     def policy_update(self):
@@ -627,7 +632,7 @@ class cchess_main(object):
         actions_visits = [(act, nod.N) for act, nod in self.mcts.root.child.items()]
         actions, visits = zip(*actions_visits)
         with np.errstate(divide="ignore"):
-            probs = rules.softmax(1.0 / self.temperature * np.log(visits))
+            probs = _rules.softmax(1.0 / self.temperature * np.log(visits))
         return actions, probs
 
     def get_hint(self, mcts_or_net, reverse, disp_mcts_msg_handler):
@@ -638,13 +643,13 @@ class cchess_main(object):
                 self.mcts.main(self.game_borad.state, self.game_borad.current_player, self.game_borad.restrict_round, self.playout_counts)
             actions, probs = self._visit_probs()
             for i in range(len(actions)):
-                action = "".join(rules.flipped_uci_labels(actions[i])) if self.human_color == "w" else actions[i]
+                action = "".join(_rules.flipped_uci_labels(actions[i])) if self.human_color == "w" else actions[i]
                 act_prob_dict[action] = probs[i]
         elif mcts_or_net == "net":
             moves, p, _ = self._net_priors()
             for action, mov_p in zip(moves, p):
                 if self.human_color == "w":
-                    action = "".join(rules.flipped_uci_labels(action))
+                    action = "".join(_rules.flipped_uci_labels(action))
                 act_prob_dict[action] = mov_p
         return sorted(act_prob_dict.items(), key=lambda item: item[1], reverse=reverse)
 
@@ -654,12 +659,12 @@ class cchess_main(object):
         action_probs, value = self.mcts.forward(np.expand_dims(positions, 0))
         if self.mcts.is_black_turn(self.game_borad.current_player):
             action_probs = cchess_main.flip_policy(action_probs)
-        moves = rules.GameBoard.get_legal_moves(self.game_borad.state, self.game_borad.current_player)
+        moves = _rules.GameBoard.get_legal_moves(self.game_borad.state, self.game_borad.current_player)
         action_probs = np.asarray(action_probs).flatten()
         tot_p = 1e-8
         p = []
         for action in moves:
-            mov_p = action_probs[rules.label2i[action]]
+            mov_p = action_probs[_rules.label2i[action]]
             p.append(mov_p)
             tot_p += mov_p
         return moves, [x / tot_p for x in p], value
@@ -669,9 +674,9 @@ class cchess_main(object):
         """(pseudo-legal move labels, their strict-legality flags, in check, mated) for the side to move on the board:
         one k_strict_moves launch."""
         gb = self.game_borad
-        mv, cnt, legal, chk, mated = rules.strict_moves_batch(rules.state_to_board(gb.state)[None], [rules.side_of(gb.current_player)])
+        mv, cnt, legal, chk, mated = _rules.strict_moves_batch(_rules.state_to_board(gb.state)[None], [_rules.side_of(gb.current_player)])
         n = min(int(cnt[0]), mv.shape[1])
-        return [rules.move_to_label(m) for m in mv[0, :n]], legal[0, :n], bool(chk[0]), bool(mated[0])
+        return [_rules.move_to_label(m) for m in mv[0, :n]], legal[0, :n], bool(chk[0]), bool(mated[0])
 
     def _playable(self):
         """Labels of the moves that are strictly legal and not banned."""
@@ -699,7 +704,7 @@ class cchess_main(object):
         if self.strict:
             visits = self._strict_visits(actions, visits)
         with np.errstate(divide="ignore"):
-            probs = rules.softmax(1.0 / temperature * np.log(visits))
+            probs = _rules.softmax(1.0 / temperature * np.log(visits))
         move_probs = [[actions, probs]]
         if self.exploration and self.strict:      # the Dirichlet noise must not revive a filtered move
             p = np.where(np.asarray(visits) > 0, 0.75 * probs + 0.25 * np.random.dirichlet(0.3 * np.ones(len(probs))), 0.0)
@@ -735,10 +740,10 @@ class cchess_main(object):
     def _advance(self, action):
         """state / round / player / restrict_round bookkeeping shared by human_move, select_move, selfplay."""
         last_state = self.game_borad.state
-        self.game_borad.state = rules.GameBoard.sim_do_action(action, self.game_borad.state)
+        self.game_borad.state = _rules.GameBoard.sim_do_action(action, self.game_borad.state)
         self.game_borad.round += 1
         self.game_borad.current_player = "w" if self.game_borad.current_player == "b" else "b"
-        if rules.is_kill_move(last_state, self.game_borad.state) == 0:
+        if _rules.is_kill_move(last_state, self.game_borad.state) == 0:
             self.game_borad.restrict_round += 1
         else:
             self.game_borad.restrict_round = 0
@@ -747,7 +752,7 @@ class cchess_main(object):
         win_rate = 0
         action = "abcdefghi"[coord[0]] + str(coord[1]) + "abcdefghi"[coord[2]] + str(coord[3])
         if self.human_color == "w":
-            action = "".join(rules.flipped_uci_labels(action))
+            action = "".join(_rules.flipped_uci_labels(action))
         if self.strict:
             labels, legal, _, _ = self._strict_position()
             if action not in {m for m, ok in zip(labels, legal) if ok}:
@@ -775,7 +780,7 @@ class cchess_main(object):
         self._advance(action)
         self.game_borad.print_borad(self.game_borad.state)
         if self.human_color == "w":
-            action = "".join(rules.flipped_uci_labels(action))
+            action = "".join(_rules.flipped_uci_labels(action))
         sx, sy, dx, dy = ord(action[0]) - 97, int(action[1]), ord(action[2]) - 97, int(action[3])
         return (sx, sy, dx - sx, dy - sy), win_rate
 
@@ -790,9 +795,9 @@ class cchess_main(object):
             black = self.mcts.is_black_turn(self.game_borad.current_player)
             state, _ = self.mcts.try_flip(self.game_borad.state, self.game_borad.current_player, black)
             states.append(state)
-            prob = np.zeros(rules.labels_len)
+            prob = np.zeros(_rules.labels_len)
             for a, pr in zip(probs[0][0], probs[0][1]):
-                prob[rules.label2i["".join(rules.flipped_uci_labels(a)) if black else a]] = pr
+                prob[_rules.label2i["".join(_rules.flipped_uci_labels(a)) if black else a]] = pr
             mcts_probs.append(prob)
             current_players.append(self.game_borad.current_player)
             self._advance(action)

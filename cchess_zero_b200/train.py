@@ -286,10 +286,14 @@ class Trainer:
 
     def __init__(self, network, n_games, playouts, search_threads=1, batch_size=512, buffer_size=10000, epochs=5, kl_targ=0.025,
                  learning_rate=1e-3, updates_per_game=1, mirror=False, eval_every=0, eval_games=10, eval_playouts=None,
-                 gate_threshold=0.55, checkpoint_every=100, seed=0, arena_words=1 << 20, best=None):
+                 gate_threshold=0.55, checkpoint_every=100, seed=0, arena_words=1 << 20, best=None, rules="reference"):
+        """rules: 'reference' or 'strict' -- self-play and the gate's matches search strictly legal moves only and a side without
+        one is mated (the network learns the full rules of xiangqi); strict rules need search_threads = 1."""
+        from .engine import check_rules
         from .selfplay import network_selfplay
         if eval_every and (eval_games <= 0 or eval_games % 2):
             raise ValueError("eval_games must be a positive even number (colour-swapped pairs)")
+        self.rules = check_rules(rules, search_threads)
         self.network = network
         self.n_games, self.playouts, self.search_threads = int(n_games), playouts, int(search_threads)
         self.batch_size, self.epochs, self.kl_targ = int(batch_size), int(epochs), kl_targ
@@ -305,7 +309,8 @@ class Trainer:
             self.best = best if best is not None else _clone_network(network, os.path.join(network.save_dir, "best"))
         self.buffer = ReplayBuffer(buffer_size, network.device.index)
         self.sp = network_selfplay(self.best or network, self.n_games, playouts, seeds=[self.seed * self.n_games + g for g in range(self.n_games)],
-                                   search_threads=self.search_threads, arena_words=arena_words, auto_reset=True, keep_records=True)
+                                   search_threads=self.search_threads, arena_words=arena_words, auto_reset=True, keep_records=True,
+                                   rules=self.rules)
         self.sp.capture_graph()
         self.games = self.positions = self.updates = self.train_steps = self.promotions = self.gates = self.plies = 0
         self.next_gate = self.eval_every
@@ -355,7 +360,7 @@ class Trainer:
         from .arena import Match
         g0 = self.gates * self.eval_games
         r = Match(self.network, self.best, self.eval_games, self.eval_playouts, search_threads=self.search_threads,
-                  seeds=range(g0, g0 + self.eval_games), arena_words=self.arena_words).run()
+                  seeds=range(g0, g0 + self.eval_games), arena_words=self.arena_words, rules=self.rules).run()
         self.gates += 1
         self.last_gate = json.loads(r.to_json(self.gate_threshold, games=False))
         if r.promote(self.gate_threshold):
@@ -432,7 +437,7 @@ class Trainer:
         version, internal, gauss = self.rng.getstate()
         _savez(os.path.join(directory, "trainer.npz"), rng_version=version, rng_internal=np.asarray(internal, dtype=np.uint32),
                rng_gauss=np.float64(0.0 if gauss is None else gauss), rng_has_gauss=gauss is not None, mt=self.sp._mt,
-               lr_multiplier=self.lr_multiplier, next_gate=self.next_gate,
+               lr_multiplier=self.lr_multiplier, next_gate=self.next_gate, rules=np.asarray(self.rules),
                counters=np.asarray([self.games, self.positions, self.updates, self.train_steps, self.promotions, self.gates, self.plies],
                                    dtype=np.int64))
         self.sp.save_games(os.path.join(directory, "games.npz"))
@@ -442,6 +447,9 @@ class Trainer:
         with np.load(os.path.join(directory, "trainer.npz"), allow_pickle=False) as d:
             if d["mt"].shape != self.sp._mt.shape:
                 raise ValueError("saved run has %d game slots, this Trainer %d" % (d["mt"].shape[0], self.n_games))
+            saved = str(d["rules"]) if "rules" in d.files else "reference"          # (runs saved before the rules choice existed)
+            if saved != self.rules:
+                raise ValueError("saved run plays by the %r rules, this Trainer by %r" % (saved, self.rules))
             gauss = float(d["rng_gauss"]) if bool(d["rng_has_gauss"]) else None
             self.rng.setstate((int(d["rng_version"]), tuple(int(v) for v in d["rng_internal"]), gauss))
             mt = d["mt"].copy()
@@ -496,6 +504,8 @@ def main(argv=None):
     ap.add_argument("--mirror", action="store_true", help="mirror a random half of every mini-batch left to right")
     ap.add_argument("--save-dir", required=True, help="checkpoints and the state a --resume continues from")
     ap.add_argument("--resume", action="store_true", help="continue the run saved in --save-dir")
+    ap.add_argument("--rules", choices=("reference", "strict"), default="reference",
+                    help="strict: search strictly legal moves only; a side without one is mated (needs --search-threads 1)")
     a = ap.parse_args(argv)
     from .net import policy_value_network
     out = sys.stdout
@@ -506,7 +516,7 @@ def main(argv=None):
         t = Trainer(net, a.games, a.playouts, search_threads=a.search_threads, batch_size=a.batch_size, buffer_size=a.buffer_size,
                     epochs=a.epochs, learning_rate=a.learning_rate, updates_per_game=a.updates_per_game, mirror=a.mirror,
                     eval_every=a.eval_every, eval_games=a.eval_games, eval_playouts=a.eval_playouts, gate_threshold=a.gate_threshold,
-                    checkpoint_every=a.checkpoint_every, seed=a.seed)
+                    checkpoint_every=a.checkpoint_every, seed=a.seed, rules=a.rules)
         if t.best is not None:
             t.best.save_dir = os.path.join(a.save_dir, "best")
         if a.resume and os.path.isfile(os.path.join(a.save_dir, "trainer.npz")):

@@ -136,6 +136,22 @@ int cz_engine_create_ex(int n_games, int64_t arena_words, int device, int leaves
 int cz_engine_create_fifo(int n_games, int64_t arena_words, int device, int search_threads, cz_engine **out);
 int cz_engine_is_fifo(const cz_engine *e);
 int cz_engine_leaves(const cz_engine *e);
+/* A one-leaf engine (cz_engine_create) that plays by the given rules.
+ *   CZ_RULES_REFERENCE: the reference's rules (pseudo-legal moves; a game ends when a king is taken): cz_engine_create's engine.
+ *   CZ_RULES_STRICT:    the full rules of xiangqi.  A node's children are its strictly legal moves (the subset of the pseudo-legal
+ *                       list that leaves the mover's king unattacked, cz_strict_moves_batch, in the same order; priors normalised over
+ *                       them).  A node without one is mated (checkmate and stalemate both lose): it is expanded with no children, the
+ *                       playout that expanded it backs up as if the network had returned -1 for the side to move there, and later
+ *                       descents onto it end there worth +1 to the move into it.  A root without a strictly legal move ends the game
+ *                       with terminal code 3 after cz_engine_reset / set_root_meta / play / play_moves (one extra kernel launch each);
+ *                       cz_engine_play_moves on an unexpanded root accepts only strictly legal moves among the first 128 pseudo-legal
+ *                       ones (the moves an expansion keeps; more than 128 is CZ_ERR_CHILDREN, possible on set-up boards only).  A king capture stays legal and
+ *                       terminal (set-up positions only).  Snapshots are written in format 2.
+ * Any other value: CZ_EINVAL.  Leaf-parallel and search_threads = K engines play by the reference rules only. */
+#define CZ_RULES_REFERENCE 0
+#define CZ_RULES_STRICT 1
+int cz_engine_create_rules(int n_games, int64_t arena_words, int device, int rules, cz_engine **out);
+int cz_engine_rules(const cz_engine *e);
 int cz_engine_destroy(cz_engine *e);
 int cz_engine_n_games(const cz_engine *e);
 
@@ -201,7 +217,8 @@ int cz_engine_root_children(cz_engine *e, void *stream, int32_t *n_children /* [
  * (main.py:1532-1545).  child_index is a HOST buffer. */
 int cz_engine_play(cz_engine *e, void *stream, const int32_t *child_index /* [B] */);
 /* Same, and returns every game's packed status record (one kernel, one device->host copy, one synchronisation):
- * CZ_STATUS_BYTES per game: [0,90) board | 90 side | 91 terminal | 92 winner (int8) | 96 ply i32 | 100 restrict_round i32 |
+ * CZ_STATUS_BYTES per game: [0,90) board | 90 side | 91 terminal (codes of cz_engine_status) | 92 winner (int8) | 96 ply i32 |
+ * 100 restrict_round i32 |
  * 104 Q (f32) of the move just played = MCTS_tree.Q(act), main.py:1350 | 108 N of the new root i32. */
 #define CZ_STATUS_BYTES 112
 int cz_engine_play_status(cz_engine *e, void *stream, const int32_t *child_index /* [B] */, uint8_t *status /* host [B][112] or NULL */);
@@ -217,7 +234,8 @@ int cz_engine_play_moves(cz_engine *e, void *stream, const uint16_t *moves /* [B
 int cz_engine_status_packed(cz_engine *e, void *stream, uint8_t *status /* host [B][112] */);
 
 /* Game status (cchess_main.check_end main.py:1380-1392): HOST buffers, any may be NULL; synchronises.
- * terminal: 0 running, 1 king captured, 2 draw (restrict_round >= 60); winner: 0 'w', 1 'b', -1 none. */
+ * terminal: 0 running, 1 king captured, 2 draw (restrict_round >= 60), 3 mated (strict engines: the side to move has no strictly
+ * legal move; the winner is the side that just moved); winner: 0 'w', 1 'b', -1 none. */
 int cz_engine_status(cz_engine *e, void *stream, uint8_t *terminal, int8_t *winner, int32_t *ply, int32_t *rr,
                      uint8_t *side, uint8_t *boards /* [B][90] */);
 
@@ -236,14 +254,15 @@ int cz_engine_tree_signature(cz_engine *e, void *stream, int game, int64_t *out,
  * returned 0, after cz_engine_play, after a reset).  Its whole state is then its 16-word header line, its root board, its five
  * counters, its FIFO event-loop words (cz_engine_create_fifo engines) and words [0, alloc) of its current arena half (the live tree:
  * cz_engine_play compacts it to offset 0).  Blob layout (little-endian, 4-byte words):
- *   head  u64 [6]: magic 0x485350414E535A43 ("CZSNAPSH") | format 1 (low 32 bits), cz_version() (high) | FNV-1a 64 checksum of the
+ *   head  u64 [6]: magic 0x485350414E535A43 ("CZSNAPSH") | format (low 32 bits: 1 = reference rules, 2 = strict rules, same layout),
+ *                  cz_version() (high) | FNV-1a 64 checksum of the
  *                  Zobrist key table | n_games (low), leaves K (high) | narr = arrays per node block, 5 or 6 (low), F (high)
  *   off   i64 [n_games + 1]: word offset of every game's section and of the end; head + off padded to a multiple of 16 bytes
  *   per game: hdr [16] | root board [24] (96 bytes) | counters u64 [5] (expand, playout, L, c, C) | pad [2] | fifo [28] (narr 6
  *             only) | arena [alloc]  -- F = 52 (narr 5) or 80 (narr 6) words precede the arena, alloc = hdr[7]
  * cz_engine_snapshot_size: the blob's size in bytes (synchronises stream).  cz_engine_snapshot: writes it to out (host, cap bytes;
  * *bytes = its size), one pack kernel and one device->host copy.  Both return CZ_EINVAL when a game is not at rest, snapshot also
- * when cap is too small.  cz_engine_restore: validates the whole blob first (cz_snapshot_check against this engine) and returns
+ * when cap is too small.  cz_engine_restore: validates the whole blob first (cz_snapshot_check_rules against this engine) and returns
  * CZ_EINVAL naming the game and the failed check with the engine untouched; otherwise one host->device copy and one unpack
  * kernel write it IN PLACE into the engine's buffers (captured CUDA graphs stay valid) and every game is at rest.  The arena size
  * may differ from the saving engine's as long as every alloc fits.  Board hashing on / off is not part of a snapshot. */
@@ -255,8 +274,14 @@ int cz_engine_restore(cz_engine *e, void *stream, const void *in /* host */, int
  * <= arena_words and a multiple of 8, header at rest with valid flag / terminal / winner codes, root child count in {-1, 0..128},
  * root board piece codes 0..14, FIFO loop at rest; every block reachable from the root lies in [0, alloc), 8-word aligned, with a
  * header count equal to its parent's META n_grandchildren and <= 128, blocks disjoint, child pointers above their parent's base,
- * move squares < 90, META bits 24-31 clear.  CZ_OK or CZ_EINVAL (cz_last_error names the game and the check). */
+ * move squares < 90, META bits 24-31 clear.  CZ_OK or CZ_EINVAL (cz_last_error names the game and the check).  This is the check for
+ * a reference-rules engine: format 1 only. */
 int cz_snapshot_check(const void *in, int64_t bytes, int n_games, int leaves, int narr, int64_t arena_words);
+/* The same checks for an engine of the given rules: CZ_RULES_REFERENCE is cz_snapshot_check; CZ_RULES_STRICT accepts format 2 only,
+ * where terminal code 3 and mated nodes (an expanded child with n_grandchildren 0, or a root with count 0) may occur, each as a bare
+ * 8-word block (the words after it end the tree or start another reachable block).  A blob of the other rules' format is refused
+ * ("rules differ").  cz_engine_restore runs this with the engine's rules. */
+int cz_snapshot_check_rules(const void *in, int64_t bytes, int n_games, int leaves, int narr, int64_t arena_words, int rules);
 
 /* ---- network ends (policy_value_network.py:45-48 and 55-74), hand-written; the residual tower is library code ----
  * cz_net_first_conv: canonical boards (dev u8 [B][96], from cz_engine_wave with CZ_BOARD) ->
