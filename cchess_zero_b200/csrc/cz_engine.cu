@@ -36,6 +36,7 @@
 
 #include <string>
 #include <vector>
+#include <type_traits>
 
 #include "../../include/cchess_b200.h"
 #include "cz_rules.cuh"
@@ -203,11 +204,31 @@ __device__ void warp_backup_path(const uint2 *path, uint32_t *ar, int depth, flo
 
 // Move list of the leaf staged in S.board (+ side in byte 90), in reference order, and the label index of every move (with
 // flip_policy, main.py:1152-1155, folded into the index: rank y -> 9-y for black).  Leaves S.moves[i] / S.li[i]; returns n.
+// STRICT (k_wave<T, true>): only the strictly legal moves.  warp_strict_moves' list is compacted onto S.moves in move-generation
+// order (ballot + popcount of the legal mask); zero strictly legal moves is a mated position, not an error.
+template <bool STRICT>
 __device__ int warp_leaf_moves(const Dev &E, WarpSmem &S, uint32_t &errf, int lane) {
     const int lside = S.board[90];
-    int n = cz::warp_legal_moves(S.board, lside, S.moves, S.scratch, lane);
-    if (n == 0) errf |= CZ_ERR_NOMOVES;
+    uint32_t legal[4];
+    int fl, n;
+    if constexpr (STRICT) n = cz::warp_strict_moves(S.board, lside, S.moves, S.scratch, lane, legal, fl);
+    else n = cz::warp_legal_moves(S.board, lside, S.moves, S.scratch, lane);
+    if (!STRICT && n == 0) errf |= CZ_ERR_NOMOVES;
     if (n > CZ_MAXCHILD) { errf |= CZ_ERR_CHILDREN; n = CZ_MAXCHILD; }
+    if constexpr (STRICT) {
+        uint16_t mv[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++) { const int i = lane + 32 * k; mv[k] = i < n ? S.moves[i] : (uint16_t)0; }
+        __syncwarp();
+        const uint32_t below = (1u << lane) - 1u;
+        n = 0;
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            if ((legal[k] >> lane) & 1u) S.moves[n + __popc(legal[k] & below)] = mv[k];
+            n += __popc(legal[k]);
+        }
+        __syncwarp();
+    }
     for (int i = lane; i < n; i += 32) {
         const int mv = S.moves[i];
         int src = mv & 127, dst = mv >> 7;
@@ -225,63 +246,17 @@ __device__ int warp_leaf_moves(const Dev &E, WarpSmem &S, uint32_t &errf, int la
 
 // leaf_node.expand (main.py:175-187) in three parts.
 // 1: move generation + arena reservation.  Returns n > 0, or 0 when the expansion cannot happen (no moves / arena full).
+// STRICT: returns n >= 0 (0 = mated: the reservation is the bare 8-word header), or -1 when the arena is full.
+template <bool STRICT>
 __device__ int expand_reserve(const Dev &E, WarpSmem &S, uint32_t &alloc, uint32_t &base, uint32_t &errf, int lane) {
     uint32_t ef = 0;
-    const int n = warp_leaf_moves(E, S, ef, lane);
+    const int n = warp_leaf_moves<STRICT>(E, S, ef, lane);
     const uint32_t cs = (uint32_t)((n + 7) & ~7), size = HDR + (uint32_t)E.narr * cs;
     base = alloc;
     if ((long long)base + size > E.A) ef |= CZ_ERR_ARENA;
     ef = __reduce_or_sync(CZ_FULL, ef);
     errf |= ef;
-    if (ef & (CZ_ERR_ARENA | CZ_ERR_NOMOVES)) return 0;
-    alloc = base + size;
-    return n;
-}
-// Strict rules (k_wave<T, true>): parts 0 and 1 over the strictly legal moves.  warp_strict_moves' list is compacted onto
-// S.moves in move-generation order (ballot + popcount of the legal mask), then labelled as warp_leaf_moves does.  Zero strictly
-// legal moves is a mated position, not an error: the reservation is then the bare 8-word header.  Returns n >= 0, or -1 when the
-// arena is full.
-__device__ int warp_leaf_moves_strict(const Dev &E, WarpSmem &S, uint32_t &errf, int lane) {
-    const int lside = S.board[90];
-    uint32_t legal[4];
-    int fl;
-    int n = cz::warp_strict_moves(S.board, lside, S.moves, S.scratch, lane, legal, fl);
-    if (n > CZ_MAXCHILD) { errf |= CZ_ERR_CHILDREN; n = CZ_MAXCHILD; }
-    uint16_t mv[4];
-#pragma unroll
-    for (int k = 0; k < 4; k++) { const int i = lane + 32 * k; mv[k] = i < n ? S.moves[i] : (uint16_t)0; }
-    __syncwarp();
-    const uint32_t below = (1u << lane) - 1u;
-    int m = 0;
-#pragma unroll
-    for (int k = 0; k < 4; k++) {
-        if ((legal[k] >> lane) & 1u) S.moves[m + __popc(legal[k] & below)] = mv[k];
-        m += __popc(legal[k]);
-    }
-    __syncwarp();
-    for (int i = lane; i < m; i += 32) {
-        const int v = S.moves[i];
-        int src = v & 127, dst = v >> 7;
-        if (lside == 1) {
-            src = (9 - src / 9) * 9 + src % 9;
-            dst = (9 - dst / 9) * 9 + dst % 9;
-        }
-        int li = __ldg(E.label_of + src * CZ_NSQ + dst);
-        if (li < 0) { errf |= CZ_ERR_NOLABEL; li = 0; }
-        S.li[i] = (uint16_t)li;
-    }
-    __syncwarp();
-    return m;
-}
-__device__ int expand_reserve_strict(const Dev &E, WarpSmem &S, uint32_t &alloc, uint32_t &base, uint32_t &errf, int lane) {
-    uint32_t ef = 0;
-    const int n = warp_leaf_moves_strict(E, S, ef, lane);
-    const uint32_t cs = (uint32_t)((n + 7) & ~7), size = HDR + (uint32_t)E.narr * cs;
-    base = alloc;
-    if ((long long)base + size > E.A) ef |= CZ_ERR_ARENA;
-    ef = __reduce_or_sync(CZ_FULL, ef);
-    errf |= ef;
-    if (ef & CZ_ERR_ARENA) return -1;
+    if (ef & (STRICT ? CZ_ERR_ARENA : CZ_ERR_ARENA | CZ_ERR_NOMOVES)) return STRICT ? -1 : 0;
     alloc = base + size;
     return n;
 }
@@ -409,6 +384,39 @@ __device__ __forceinline__ uint32_t select_child(const BlockRegs &R, int cnt, in
     return __reduce_min_sync(CZ_FULL, (bi != NONE && hi == mhi && lo == mlo) ? bi : NONE);
 }
 
+// The edge select_child picks, with the owner lane / register slot of its entry and its META, CHILD and N on every lane.
+struct Edge {
+    uint32_t e;
+    int owner, ke;
+    uint32_t meta, child;
+    int N;
+};
+template <int MODE>
+__device__ __forceinline__ Edge select_edge(const BlockRegs &R, int cnt, int parentN, int lane) {
+    const uint32_t e = select_child<MODE>(R, cnt, parentN, lane);
+    const int owner = e & 31, ke = (int)(e >> 5);
+    return {e, owner, ke, __shfl_sync(CZ_FULL, pick(R.meta, ke), owner), __shfl_sync(CZ_FULL, pick(R.child, ke), owner),
+            (int)__shfl_sync(CZ_FULL, pick(R.N, ke), owner)};
+}
+
+// Plays a move on the board staged in S.board once every lane has read the board (the caller reads the captured piece and the
+// mover itself: reading them here instead changes how k_wave computes the Zobrist addresses of the move).
+__device__ __forceinline__ void play_move(WarpSmem &S, int src, int dst, int mover, int lane) {
+    __syncwarp();
+    if (lane == 0) { S.board[dst] = (uint8_t)mover; S.board[src] = 0; }
+    __syncwarp();
+}
+// Stages a board (24 words, lane l < 24 holding word l) in the warp's shared memory.
+__device__ __forceinline__ void stage_board(WarpSmem &S, uint32_t word, int lane) {
+    if (lane < 24) reinterpret_cast<uint32_t *>(S.board)[lane] = word;
+    __syncwarp();
+}
+// (row `row` of a [rows][96] array: the address is formed on the lanes that load)
+__device__ __forceinline__ void stage_board(WarpSmem &S, const uint8_t *boards, size_t row, int lane) {
+    if (lane < 24) reinterpret_cast<uint32_t *>(S.board)[lane] = reinterpret_cast<const uint32_t *>(boards + row * 96)[lane];
+    __syncwarp();
+}
+
 #define HGET(f) __shfl_sync(CZ_FULL, h, (f))
 #define HSET(f, v) do { if (lane == (f)) h = (uint32_t)(v); } while (0)
 
@@ -456,12 +464,9 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave(Dev E, T *nn_in, const
         // ---- round trip 2: the W / N words of the path (back-up operands) fly under the move generation ----
         uint32_t bW = 0, bN = 0;
         if (lane < depth && lane < SPATH) { bW = ar[pth.x + PE_CS(pth)]; bN = ar[pth.x + 2 * PE_CS(pth)]; }
-        if (lane < 24) reinterpret_cast<uint32_t *>(S.board)[lane] = lbw;
-        __syncwarp();
+        stage_board(S, lbw, lane);
         uint32_t base;
-        int n;
-        if constexpr (STRICT) n = expand_reserve_strict(E, S, alloc, base, errf, lane);
-        else n = expand_reserve(E, S, alloc, base, errf, lane);
+        const int n = expand_reserve<STRICT>(E, S, alloc, base, errf, lane);
         const bool ok = STRICT ? n >= 0 : n > 0;
         if (pend == 1) {
             // leaf returns -v (main.py:384); on an engine error the playout is closed with 0
@@ -516,8 +521,7 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave(Dev E, T *nn_in, const
         if (E.hash_on) rhash = (unsigned long long)HGET(H_HASHLO) | ((unsigned long long)HGET(H_HASHHI) << 32);
         if (root_cnt < 0) {
             // MCTS_tree.main: expand the root first (main.py:475-487); not a playout
-            if (lane < 24) reinterpret_cast<uint32_t *>(S.board)[lane] = rbw;
-            __syncwarp();
+            stage_board(S, rbw, lane);
             store_leaf_at<T>(E.leaf_board + (size_t)g * 96, S, side0, nn_in, (size_t)g, lane);
             if (E.hash_on && lane == 0) E.leaf_hash[g] = rhash;
             pend = 2; plen = 0;
@@ -529,8 +533,7 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave(Dev E, T *nn_in, const
             int budget = MAX_INKERNEL_PLAYOUTS;
             while (done < target && budget-- > 0) {
                 // ---- one playout of start_tree_search (main.py:350-440) ----
-                if (lane < 24) reinterpret_cast<uint32_t *>(S.board)[lane] = rbw;
-                __syncwarp();
+                stage_board(S, rbw, lane);
                 int side = side0, rr = rr0, depth = 0;
                 uint32_t base = root_base;
                 int cnt = root_cnt;
@@ -548,30 +551,26 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave(Dev E, T *nn_in, const
                     }
                     const uint32_t cs = (uint32_t)((cnt + 7) & ~7);
                     uint32_t *blk = ar + base + HDR;
-                    const uint32_t e = select_child<0>(R, cnt, parentN, lane);
-                    const int owner = e & 31, ke = (int)(e >> 5);
-                    const uint32_t meta = __shfl_sync(CZ_FULL, pick(R.meta, ke), owner);
-                    const uint32_t child = __shfl_sync(CZ_FULL, pick(R.child, ke), owner);
-                    const int eN = (int)__shfl_sync(CZ_FULL, pick(R.N, ke), owner);
-                    if (lane == owner) {  // virtual loss (main.py:403-404)
-                        blk[cs + e] = __float_as_uint(__fadd_rn(__uint_as_float(pick(R.W, ke)), -3.0f));
-                        blk[2 * cs + e] = (uint32_t)(eN + 3);
+                    const Edge x = select_edge<0>(R, cnt, parentN, lane);
+                    if (lane == x.owner) {  // virtual loss (main.py:403-404)
+                        blk[cs + x.e] = __float_as_uint(__fadd_rn(__uint_as_float(pick(R.W, x.ke)), -3.0f));
+                        blk[2 * cs + x.e] = (uint32_t)(x.N + 3);
                     }
                     if (lane == 0) {
-                        const uint2 pe = path_entry(base + HDR + e, cs, meta & 0xFFFFu);
+                        const uint2 pe = path_entry(base + HDR + x.e, cs, x.meta & 0xFFFFu);
                         E.path[(size_t)g * MAXD + depth] = pe;
                         if (depth < SPATH) S.path[depth] = pe;
                     }
                     depth++;
                     accL += 1; accC += (unsigned)cnt;
-                    const int src = meta & 127, dst = (meta >> 7) & 127;
+                    const int src = x.meta & 127, dst = (x.meta >> 7) & 127;
                     const int cap = S.board[dst], mover = S.board[src];
-                    __syncwarp();
-                    if (lane == 0) { S.board[dst] = (uint8_t)mover; S.board[src] = 0; }
-                    __syncwarp();
+                    play_move(S, src, dst, mover, lane);
                     if (E.hash_on) hash ^= zob_move(E.zob, mover, cap, src, dst);
                     side ^= 1;                                   // main.py:392
                     rr = cap == 0 ? rr + 1 : 0;                  // is_kill_move, main.py:393-396
+                    // The terminal tests stay written out in each wave kernel: one shared function for them changes the register
+                    // allocation of all three.
                     if (cap == 1 || cap == 8) {                  // king captured: main.py:409-414
                         const float v = cap == 1 ? (side == 1 ? 1.0f : -1.0f) : (side == 1 ? -1.0f : 1.0f);
                         tval = -v;
@@ -579,12 +578,12 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave(Dev E, T *nn_in, const
                     }
                     if (rr >= 60) { tval = 0.0f; break; }        // main.py:415-416
                     if constexpr (STRICT) {                      // expanded without children: the side to move is mated
-                        if (child != NONE && ((meta >> 16) & 0xFFu) == 0) { tval = 1.0f; break; }
+                        if (x.child != NONE && ((x.meta >> 16) & 0xFFu) == 0) { tval = 1.0f; break; }
                     }
-                    if (child == NONE) { leaf = true; break; }   // main.py:357: not expanded -> evaluate
-                    base = child;
-                    cnt = (int)((meta >> 16) & 0xFFu);
-                    parentN = eN + 3;                            // the child's N carries the virtual loss just added
+                    if (x.child == NONE) { leaf = true; break; } // main.py:357: not expanded -> evaluate
+                    base = x.child;
+                    cnt = (int)((x.meta >> 16) & 0xFFu);
+                    parentN = x.N + 3;                           // the child's N carries the virtual loss just added
                     load_block<false>(ar, base, cnt, lane, R);   // one round trip per level: the pointer chase itself
                 }
                 if ((uint32_t)depth > maxdep) maxdep = (uint32_t)depth;
@@ -660,10 +659,9 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave_multi(Dev E, T *nn_in,
         if (!pend) continue;
         const int depth = E.plenK[idx];
         const uint2 *path = E.pathK + idx * MAXD;
-        if (lane < 24) reinterpret_cast<uint32_t *>(S.board)[lane] = reinterpret_cast<const uint32_t *>(E.leafK + idx * 96)[lane];
-        __syncwarp();
+        stage_board(S, E.leafK, idx, lane);
         uint32_t base;
-        const int n = expand_reserve(E, S, alloc, base, errf, lane);
+        const int n = expand_reserve<false>(E, S, alloc, base, errf, lane);
         const bool ok = n > 0;
         if (ok) {
             expand_write(ar, S, logits + idx * CZ_NLABEL, n, base, lane);
@@ -683,8 +681,7 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave_multi(Dev E, T *nn_in,
     }
 
     if (!dead && root_cnt < 0) {   // root expansion first (main.py:475-487), one slot
-        if (lane < 24) reinterpret_cast<uint32_t *>(S.board)[lane] = rbw;
-        __syncwarp();
+        stage_board(S, rbw, lane);
         store_leaf_at<T>(E.leafK + (size_t)g * K * 96, S, side0, nn_in, (size_t)g * K, lane);
         if (lane == 0) { E.pendK[(size_t)g * K] = 2; E.plenK[(size_t)g * K] = 0; if (E.hash_on) E.leaf_hash[(size_t)g * K] = rhash; }
     } else if (!dead) {
@@ -697,8 +694,7 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave_multi(Dev E, T *nn_in,
             const size_t idx = (size_t)g * K + s;
             uint2 *path = E.pathK + idx * MAXD;
             while (done + inflight < target && budget-- > 0) {
-                if (lane < 24) reinterpret_cast<uint32_t *>(S.board)[lane] = rbw;
-                __syncwarp();
+                stage_board(S, rbw, lane);
                 int side = side0, rr = rr0, depth = 0;
                 uint32_t base = root_base;
                 int cnt = root_cnt;
@@ -715,27 +711,22 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave_multi(Dev E, T *nn_in,
                     const uint32_t cs = (uint32_t)((cnt + 7) & ~7);
                     uint32_t *blk = ar + base + HDR;
                     load_block<false>(ar, base, cnt, lane, R);
-                    const uint32_t e = select_child<1>(R, cnt, parentN, lane);
-                    const int owner = e & 31, ke = (int)(e >> 5);
-                    const uint32_t meta = __shfl_sync(CZ_FULL, pick(R.meta, ke), owner);
-                    const uint32_t child = __shfl_sync(CZ_FULL, pick(R.child, ke), owner);
-                    const int eN = (int)__shfl_sync(CZ_FULL, pick(R.N, ke), owner);
-                    const bool claimed = (meta & 0x80000000u) != 0;
-                    const int src = meta & 127, dst = (meta >> 7) & 127;
+                    const Edge x = select_edge<1>(R, cnt, parentN, lane);
+                    const bool claimed = (x.meta & 0x80000000u) != 0;
+                    // the captured piece and the terminal test are read before the virtual loss: a terminal edge is never claimed
+                    const int src = x.meta & 127, dst = (x.meta >> 7) & 127;
                     const int cap = S.board[dst], mover = S.board[src];
                     const bool term = cap == 1 || cap == 8 || (cap == 0 ? rr + 1 : 0) >= 60;
-                    if (child == NONE && claimed && !term) { outcome = 3; break; }     // someone else is evaluating this leaf
-                    if (lane == owner) {  // virtual loss + in-flight count (+ claim when this becomes our leaf)
-                        blk[cs + e] = __float_as_uint(__fadd_rn(__uint_as_float(pick(R.W, ke)), -3.0f));
-                        blk[2 * cs + e] = (uint32_t)(eN + 3);
-                        blk[3 * cs + e] = (meta + (1u << 24)) | ((child == NONE && !term) ? 0x80000000u : 0u);
+                    if (x.child == NONE && claimed && !term) { outcome = 3; break; }     // someone else is evaluating this leaf
+                    if (lane == x.owner) {  // virtual loss + in-flight count (+ claim when this becomes our leaf)
+                        blk[cs + x.e] = __float_as_uint(__fadd_rn(__uint_as_float(pick(R.W, x.ke)), -3.0f));
+                        blk[2 * cs + x.e] = (uint32_t)(x.N + 3);
+                        blk[3 * cs + x.e] = (x.meta + (1u << 24)) | ((x.child == NONE && !term) ? 0x80000000u : 0u);
                     }
-                    if (lane == 0) path[depth] = path_entry(base + HDR + e, cs, meta & 0xFFFFu);
+                    if (lane == 0) path[depth] = path_entry(base + HDR + x.e, cs, x.meta & 0xFFFFu);
                     depth++;
                     accL += 1; accC += (unsigned)cnt;
-                    __syncwarp();
-                    if (lane == 0) { S.board[dst] = (uint8_t)mover; S.board[src] = 0; }
-                    __syncwarp();
+                    play_move(S, src, dst, mover, lane);
                     if (E.hash_on) hash ^= zob_move(E.zob, mover, cap, src, dst);
                     side ^= 1;
                     rr = cap == 0 ? rr + 1 : 0;
@@ -745,10 +736,10 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave_multi(Dev E, T *nn_in,
                         break;
                     }
                     if (rr >= 60) { tval = 0.0f; outcome = 2; break; }
-                    if (child == NONE) { outcome = 1; break; }
-                    base = child;
-                    cnt = (int)((meta >> 16) & 0xFFu);
-                    parentN = eN + 3;
+                    if (x.child == NONE) { outcome = 1; break; }
+                    base = x.child;
+                    cnt = (int)((x.meta >> 16) & 0xFFu);
+                    parentN = x.N + 3;
                 }
                 if ((uint32_t)depth > maxdep) maxdep = (uint32_t)depth;
                 __syncwarp();
@@ -862,10 +853,11 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave_fifo(Dev E, T *nn_in, 
     bool dead = false;
 
     if (pend == 2) {       // the root's evaluation arrived (main.py:475-487; its value is discarded)
+        // (staged inline: stage_board here changes this kernel's register allocation)
         if (lane < 24) reinterpret_cast<uint32_t *>(S.board)[lane] = reinterpret_cast<const uint32_t *>(E.leafK + (size_t)g * K * 96)[lane];
         __syncwarp();
         uint32_t base;
-        const int n = expand_reserve(E, S, alloc, base, errf, lane);
+        const int n = expand_reserve<false>(E, S, alloc, base, errf, lane);
         if (n > 0) {
             expand_write(ar, S, logits + NN_ROW((size_t)g * K) * CZ_NLABEL, n, base, lane, true);
             root_base = base; root_cnt = n;
@@ -873,9 +865,9 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave_fifo(Dev E, T *nn_in, 
         } else { flags &= ~F_ACTIVE; dead = true; }
         pend = 0;
     }
+    // This kernel writes no leaf_hash: an engine with search_threads keeps its keys at zero even with hashing enabled.
     if (!dead && root_cnt < 0) {
-        if (lane < 24) reinterpret_cast<uint32_t *>(S.board)[lane] = rbw;
-        __syncwarp();
+        stage_board(S, rbw, lane);
         store_leaf_at<T>(E.leafK + (size_t)g * K * 96, S, side0, nn_in, (size_t)g * K, lane);
         pend = 2; live = 1u;
     } else if (!dead) {
@@ -900,10 +892,9 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave_fifo(Dev E, T *nn_in, 
                 int plen = E.plenK[idx];
                 bool ended = false;
                 if (kind == (int)EV_RESUME) {
-                    if (lane < 24) reinterpret_cast<uint32_t *>(S.board)[lane] = reinterpret_cast<const uint32_t *>(E.leafK + idx * 96)[lane];
-                    __syncwarp();
+                    stage_board(S, E.leafK, idx, lane);
                     uint32_t base;
-                    const int n = expand_reserve(E, S, alloc, base, errf, lane);
+                    const int n = expand_reserve<false>(E, S, alloc, base, errf, lane);
                     if (n > 0) {
                         expand_write(ar, S, logits + NN_ROW(idx) * CZ_NLABEL, n, base, lane, true);
                         if (lane == 0) {
@@ -922,11 +913,10 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave_fifo(Dev E, T *nn_in, 
                     uint32_t base;
                     bool go = true;
                     if (plen == 0) {          // a fresh playout: start_tree_search(root)
-                        if (lane < 24) reinterpret_cast<uint32_t *>(S.board)[lane] = rbw;
+                        if (lane < 24) reinterpret_cast<uint32_t *>(S.board)[lane] = rbw;      // (synchronised below with the other branch)
                         side = side0; rr = rr0; base = root_base; cnt = root_cnt; parentN = root_N;
                     } else {                  // re-check after a spin: the node this task stands on
-                        if (lane < 24) reinterpret_cast<uint32_t *>(S.board)[lane] = reinterpret_cast<const uint32_t *>(E.leafK + idx * 96)[lane];
-                        __syncwarp();
+                        stage_board(S, E.leafK, idx, lane);
                         side = S.board[90]; rr = S.board[91];
                         const uint2 pe = path[plen - 1];
                         const uint32_t meta = ar[pe.x + 3 * PE_CS(pe)], child = ar[pe.x + 4 * PE_CS(pe)];
@@ -946,23 +936,17 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave_fifo(Dev E, T *nn_in, 
                         const uint32_t cs = (uint32_t)((cnt + 7) & ~7);
                         uint32_t *blk = ar + base + HDR;
                         load_block<true>(ar, base, cnt, lane, R);
-                        const uint32_t c = select_child<2>(R, cnt, parentN, lane);
-                        const int owner = c & 31, ke = (int)(c >> 5);
-                        const uint32_t meta = __shfl_sync(CZ_FULL, pick(R.meta, ke), owner);
-                        const uint32_t child = __shfl_sync(CZ_FULL, pick(R.child, ke), owner);
-                        const int eN = (int)__shfl_sync(CZ_FULL, pick(R.N, ke), owner);
-                        if (lane == owner) {  // virtual loss (main.py:403-404); Q stays as stored
-                            blk[cs + c] = __float_as_uint(__fadd_rn(__uint_as_float(pick(R.W, ke)), -3.0f));
-                            blk[2 * cs + c] = (uint32_t)(eN + 3);
+                        const Edge x = select_edge<2>(R, cnt, parentN, lane);
+                        if (lane == x.owner) {  // virtual loss (main.py:403-404); Q stays as stored
+                            blk[cs + x.e] = __float_as_uint(__fadd_rn(__uint_as_float(pick(R.W, x.ke)), -3.0f));
+                            blk[2 * cs + x.e] = (uint32_t)(x.N + 3);
                         }
-                        if (lane == 0) path[plen] = path_entry(base + HDR + c, cs, meta & 0xFFFFu);
+                        if (lane == 0) path[plen] = path_entry(base + HDR + x.e, cs, x.meta & 0xFFFFu);
                         plen++;
                         accL += 1; accC += (unsigned)cnt;
-                        const int src = meta & 127, dst = (meta >> 7) & 127;
+                        const int src = x.meta & 127, dst = (x.meta >> 7) & 127;
                         const int cap = S.board[dst], mover = S.board[src];
-                        __syncwarp();
-                        if (lane == 0) { S.board[dst] = (uint8_t)mover; S.board[src] = 0; }
-                        __syncwarp();
+                        play_move(S, src, dst, mover, lane);
                         side ^= 1;
                         rr = cap == 0 ? rr + 1 : 0;
                         if (cap == 1 || cap == 8) {                                      // main.py:409-414
@@ -972,7 +956,7 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave_fifo(Dev E, T *nn_in, 
                         }
                         if (rr >= 60) { warp_unwind_q(path, ar, plen, 0.0f, lane); ended = true; break; }   // 415-416
                         // start_tree_search(child): now_expanding? unexpanded? (main.py:354-357)
-                        if (meta & 0x80000000u) {
+                        if (x.meta & 0x80000000u) {
                             if (lane == 0) { S.board[90] = (uint8_t)side; S.board[91] = (uint8_t)rr; }
                             __syncwarp();
                             if (lane < 24) reinterpret_cast<uint32_t *>(E.leafK + idx * 96)[lane] = reinterpret_cast<const uint32_t *>(S.board)[lane];
@@ -980,15 +964,15 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave_fifo(Dev E, T *nn_in, 
                             nnxt++;
                             break;
                         }
-                        if (child == NONE) {
-                            if (lane == 0) { blk[3 * cs + c] = meta | 0x80000000u; queue[nq] = (uint8_t)slot; S.board[91] = (uint8_t)rr; }
+                        if (x.child == NONE) {
+                            if (lane == 0) { blk[3 * cs + x.e] = x.meta | 0x80000000u; queue[nq] = (uint8_t)slot; S.board[91] = (uint8_t)rr; }
                             nq++;
                             store_leaf_at<T>(E.leafK + idx * 96, S, side, nn_in, idx, lane);   // features queued (push_queue, main.py:362-366)
                             break;
                         }
-                        base = child;
-                        cnt = (int)((meta >> 16) & 0xFFu);
-                        parentN = eN + 3;
+                        base = x.child;
+                        cnt = (int)((x.meta >> 16) & 0xFFu);
+                        parentN = x.N + 3;
                     }
                     if ((uint32_t)plen > maxdep) maxdep = (uint32_t)plen;
                 }
@@ -2017,45 +2001,32 @@ int cz_engine_begin_search(cz_engine *e, void *stream, const uint8_t *mask, int 
     return CZ_OK;
 }
 
+extern "C++" {
+// Calls launch(in) with nn_in typed as the element type of network input format nn_dtype (CZ_BOARD: the 96-byte board rows).
+template <typename Launch>
+int launch_nn_typed(int nn_dtype, void *nn_in, Launch launch) {
+    if (nn_dtype == CZ_F32) launch((float *)nn_in);
+    else if (nn_dtype == CZ_BF16) launch((__nv_bfloat16 *)nn_in);
+    else if (nn_dtype == CZ_F16) launch((__half *)nn_in);
+    else if (nn_dtype == CZ_BOARD) launch((uint8_t *)nn_in);
+    else return fail(CZ_EINVAL, "wave: nn_dtype");
+    CUDA_TRY(cudaGetLastError());
+    return CZ_OK;
+}
+}
+
 int cz_engine_wave(cz_engine *e, void *stream, void *nn_in, int nn_dtype, const float *logits, const float *value) {
     if (!e || !nn_in || !logits || !value) return fail(CZ_EINVAL, "cz_engine_wave: null");
     dim3 gr(nblk(e->d.B, e->wpb)), bl(32 * e->wpb);
     const size_t sm = (size_t)e->wpb * sizeof(WarpSmem);
     cudaStream_t st = (cudaStream_t)stream;
-    if (e->d.fifo) {    // search_threads = K schedule of the reference (canonical FIFO form)
-        if (nn_dtype == CZ_F32) k_wave_fifo<float><<<gr, bl, sm, st>>>(e->d, (float *)nn_in, logits, value);
-        else if (nn_dtype == CZ_BF16) k_wave_fifo<__nv_bfloat16><<<gr, bl, sm, st>>>(e->d, (__nv_bfloat16 *)nn_in, logits, value);
-        else if (nn_dtype == CZ_F16) k_wave_fifo<__half><<<gr, bl, sm, st>>>(e->d, (__half *)nn_in, logits, value);
-        else if (nn_dtype == CZ_BOARD) k_wave_fifo<uint8_t><<<gr, bl, sm, st>>>(e->d, (uint8_t *)nn_in, logits, value);
-        else return fail(CZ_EINVAL, "wave: nn_dtype");
-        CUDA_TRY(cudaGetLastError());
-        return CZ_OK;
-    }
-    if (e->d.pendK) {   // leaf-parallel engine
-        if (nn_dtype == CZ_F32) k_wave_multi<float><<<gr, bl, sm, st>>>(e->d, (float *)nn_in, logits, value);
-        else if (nn_dtype == CZ_BF16) k_wave_multi<__nv_bfloat16><<<gr, bl, sm, st>>>(e->d, (__nv_bfloat16 *)nn_in, logits, value);
-        else if (nn_dtype == CZ_F16) k_wave_multi<__half><<<gr, bl, sm, st>>>(e->d, (__half *)nn_in, logits, value);
-        else if (nn_dtype == CZ_BOARD) k_wave_multi<uint8_t><<<gr, bl, sm, st>>>(e->d, (uint8_t *)nn_in, logits, value);
-        else return fail(CZ_EINVAL, "wave: nn_dtype");
-        CUDA_TRY(cudaGetLastError());
-        return CZ_OK;
-    }
-    if (e->rules == CZ_RULES_STRICT) {
-        if (nn_dtype == CZ_F32) k_wave<float, true><<<gr, bl, sm, st>>>(e->d, (float *)nn_in, logits, value);
-        else if (nn_dtype == CZ_BF16) k_wave<__nv_bfloat16, true><<<gr, bl, sm, st>>>(e->d, (__nv_bfloat16 *)nn_in, logits, value);
-        else if (nn_dtype == CZ_F16) k_wave<__half, true><<<gr, bl, sm, st>>>(e->d, (__half *)nn_in, logits, value);
-        else if (nn_dtype == CZ_BOARD) k_wave<uint8_t, true><<<gr, bl, sm, st>>>(e->d, (uint8_t *)nn_in, logits, value);
-        else return fail(CZ_EINVAL, "wave: nn_dtype");
-        CUDA_TRY(cudaGetLastError());
-        return CZ_OK;
-    }
-    if (nn_dtype == CZ_F32) k_wave<float, false><<<gr, bl, sm, st>>>(e->d, (float *)nn_in, logits, value);
-    else if (nn_dtype == CZ_BF16) k_wave<__nv_bfloat16, false><<<gr, bl, sm, st>>>(e->d, (__nv_bfloat16 *)nn_in, logits, value);
-    else if (nn_dtype == CZ_F16) k_wave<__half, false><<<gr, bl, sm, st>>>(e->d, (__half *)nn_in, logits, value);
-    else if (nn_dtype == CZ_BOARD) k_wave<uint8_t, false><<<gr, bl, sm, st>>>(e->d, (uint8_t *)nn_in, logits, value);
-    else return fail(CZ_EINVAL, "wave: nn_dtype");
-    CUDA_TRY(cudaGetLastError());
-    return CZ_OK;
+    return launch_nn_typed(nn_dtype, nn_in, [&](auto *in) {
+        using T = std::remove_pointer_t<decltype(in)>;
+        if (e->d.fifo) k_wave_fifo<T><<<gr, bl, sm, st>>>(e->d, in, logits, value);          // search_threads = K schedule of the reference
+        else if (e->d.pendK) k_wave_multi<T><<<gr, bl, sm, st>>>(e->d, in, logits, value);   // leaf-parallel engine
+        else if (e->rules == CZ_RULES_STRICT) k_wave<T, true><<<gr, bl, sm, st>>>(e->d, in, logits, value);
+        else k_wave<T, false><<<gr, bl, sm, st>>>(e->d, in, logits, value);
+    });
 }
 // search_threads = K engines: one wave with row compaction.  nn_stage [B*K rows] receives every slot's input row as cz_engine_wave
 // would write it; nn_dense [B*K rows] receives the rows that need an evaluation, densely, in (game, slot) order; logits / value are
