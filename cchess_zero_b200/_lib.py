@@ -60,6 +60,8 @@ def _sig(L):
     L.cz_engine_unfinished.argtypes = [vp, vp, vp]
     L.cz_engine_unfinished_async.argtypes = [vp, vp, vp]
     L.cz_engine_root_children.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp]
+    L.cz_engine_root_counts.argtypes = [vp, vp, vp]
+    L.cz_engine_root_noise.argtypes = [vp, vp, vp, vp, vp, vp]
     L.cz_engine_play.argtypes = [vp, vp, vp]
     L.cz_engine_status.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp]
     L.cz_engine_counters.argtypes = [vp, vp, vp]
@@ -72,6 +74,7 @@ def _sig(L):
     L.cz_net_first_conv.argtypes = [vp, i32, vp, vp, vp, vp]
     L.cz_net_heads.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.cz_host_choose_moves.argtypes = [i32, vp, vp, vp, i32, vp, vp, vp, vp, i32]
+    L.cz_host_dirichlet.argtypes = [i32, vp, vp, vp, vp, vp, i32]
     L.cz_net_heads_tc.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.cz_net_heads_fc.argtypes = [vp, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.cz_net_epilogue_split.argtypes = [vp, vp, vp, vp, vp, vp, vp, i64, vp]

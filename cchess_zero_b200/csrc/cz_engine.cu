@@ -1401,6 +1401,26 @@ __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) k_root_mate(Dev E, const
     }
 }
 
+// ---- root exploration noise (AlphaZero's P' = (1 - eps) P + eps eta at the root of every move search) -----------------------
+// For every game with mask[g], active and an expanded root with n > 0 children: P_i <- f32(keep * f64(P_i) + eps * eta[g][i]),
+// keep = 1 - eps computed once on the host.  No renormalisation.  Only the root block's P array changes; play_child keeps only the
+// chosen subtree, so the noised block is gone after the next move.
+__global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) k_root_noise(Dev E, const uint8_t *mask, const double *eta, double keep, double eps) {
+    const int lane = threadIdx.x & 31, g = blockIdx.x * WARPS_PER_BLOCK + (threadIdx.x >> 5);
+    if (g >= E.B || (mask && !mask[g])) return;
+    const uint32_t *hp = E.hdr + (size_t)g * HW;
+    const uint32_t h = lane < HW ? hp[lane] : 0u;
+    const uint32_t flags = HGET(H_FLAGS);
+    const int cnt = (int)HGET(H_ROOTCNT);
+    if (!(flags & F_ACTIVE) || cnt <= 0) return;
+    uint32_t *P = arena_half(E, g, (flags & F_CUR) ? 1 : 0) + HGET(H_ROOTBASE) + HDR;
+    const double *x = eta + (size_t)g * CZ_MAXCHILD;
+    for (int i = lane; i < cnt; i += 32) {
+        const double p = (double)__uint_as_float(P[i]);
+        P[i] = __float_as_uint(__double2float_rn(__dadd_rn(__dmul_rn(keep, p), __dmul_rn(eps, x[i]))));
+    }
+}
+
 // ---- stateless batched rules ------------------------------------------------------------
 __global__ void __launch_bounds__(32 * WARPS_PER_BLOCK) k_legal_moves(const uint8_t *boards, const uint8_t *sides, int n, uint16_t *moves, int32_t *counts) {
     __shared__ WarpSmem smem[WARPS_PER_BLOCK];
@@ -2225,6 +2245,27 @@ int cz_engine_root_keys(cz_engine *e, void *stream, uint64_t *keys) {
     int rc = fetch_headers(e, stream);
     if (rc) return rc;
     for (int g = 0; g < e->d.B; g++) keys[g] = (uint64_t)e->h_hdr[(size_t)g * HW + H_HASHLO] | ((uint64_t)e->h_hdr[(size_t)g * HW + H_HASHHI] << 32);
+    return CZ_OK;
+}
+
+int cz_engine_root_counts(cz_engine *e, void *stream, int32_t *counts) {
+    if (!e || !counts) return fail(CZ_EINVAL, "cz_engine_root_counts: null");
+    int rc = fetch_headers(e, stream);
+    if (rc) return rc;
+    for (int g = 0; g < e->d.B; g++) counts[g] = (int32_t)e->h_hdr[(size_t)g * HW + H_ROOTCNT];
+    return CZ_OK;
+}
+
+int cz_engine_root_noise(cz_engine *e, void *stream, const uint8_t *mask, const double *eta, const double *keep_p, const double *eps_p) {
+    if (!e || !eta || !keep_p || !eps_p) return fail(CZ_EINVAL, "cz_engine_root_noise: null");
+    const double keep = *keep_p, eps = *eps_p;
+    if (!(eps >= 0.0 && eps <= 1.0) || !(keep >= 0.0 && keep <= 1.0)) return fail(CZ_EINVAL, "cz_engine_root_noise: keep and eps must lie in [0, 1]");
+    cudaStream_t st = (cudaStream_t)stream;
+    CUDA_TRY(cudaSetDevice(e->device));
+    if (mask) CUDA_TRY(cudaMemcpyAsync(e->d_mask, mask, (size_t)e->d.B, cudaMemcpyHostToDevice, st));
+    k_root_noise<<<nblk(e->d.B, WARPS_PER_BLOCK), 32 * WARPS_PER_BLOCK, 0, st>>>(e->d, mask ? e->d_mask : nullptr, eta, keep, eps);
+    CUDA_TRY(cudaGetLastError());
+    if (mask) CUDA_TRY(cudaStreamSynchronize(st));      // the host mask may be pageable and is reused by the caller
     return CZ_OK;
 }
 

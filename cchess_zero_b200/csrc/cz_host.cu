@@ -10,6 +10,7 @@
 //   choice     = cdf = cumsum(p); cdf /= cdf[-1]; searchsorted(cdf, random_sample(), side='right')                    [mtrand.pyx choice]
 //   MT19937    = genrand_int32; random_sample = ((a >> 5) * 67108864 + (b >> 6)) / 9007199254740992
 // One generator state per game slot (SelfPlay's per-game RandomState), exported from / importable into numpy.RandomState.
+// cz_host_dirichlet draws RandomState.dirichlet(alpha * ones(n)) the same way for SelfPlay's root exploration noise (any 0 < alpha < 1).
 // Host code only (built by nvcc's host compiler with -ffp-contract=off: every operation is one IEEE operation).
 #include <math.h>
 #include <stdint.h>
@@ -89,6 +90,14 @@ inline double pairwise_sum(const double *a, int n) {
     for (; i < n; i++) res += a[i];
     return res;
 }
+// RandomState.dirichlet(alpha * ones(n)) for 0 < alpha < 1 [mtrand.pyx dirichlet]: n gamma draws in order, their serial sum, then
+// each scaled by 1 / sum
+inline void dirichlet_lt1(MT &s, double alpha, int n, double *d) {
+    double acc = 0.0;
+    for (int j = 0; j < n; j++) { d[j] = legacy_gamma_lt1(s, alpha); acc = acc + d[j]; }
+    const double invacc = 1 / acc;
+    for (int j = 0; j < n; j++) d[j] = d[j] * invacc;
+}
 
 void choose_range(int g0, int g1, const uint8_t *live, const int32_t *n_children, const double *ex, int exploration, MT *mt,
                   int32_t *choice, double *probs, uint8_t *fallback) {
@@ -107,11 +116,7 @@ void choose_range(int g0, int g1, const uint8_t *live, const int32_t *n_children
         if (exploration) {
             // validity of the mixed vector is checked before any draw is consumed? No: numpy draws the Dirichlet first (argument
             // evaluation), then choice() validates p.  Mirror that order.
-            MT &s = mt[g];
-            double acc = 0.0;
-            for (int j = 0; j < n; j++) { d[j] = legacy_gamma_lt1(s, 0.3); acc = acc + d[j]; }
-            const double invacc = 1 / acc;
-            for (int j = 0; j < n; j++) d[j] = d[j] * invacc;
+            dirichlet_lt1(mt[g], 0.3, n, d);
             for (int j = 0; j < n; j++) cdf[j] = 0.75 * p[j] + 0.25 * d[j];   // the mixed p (held in cdf[] until the cumsum below)
             q = cdf;
         }
@@ -131,6 +136,27 @@ void choose_range(int g0, int g1, const uint8_t *live, const int32_t *n_children
     }
 }
 
+void dirichlet_range(int g0, int g1, const uint8_t *mask, const int32_t *n, double alpha, MT *mt, double *eta) {
+    for (int g = g0; g < g1; g++)
+        if ((!mask || mask[g]) && n[g] > 0) dirichlet_lt1(mt[g], alpha, n[g], eta + (size_t)g * CZ_MAXCHILD);
+}
+
+// run(g0, g1) over n_threads contiguous ranges of games, one thread each (at least 32 games per thread; one range runs on the caller)
+template <typename F>
+void over_games(int n_games, int n_threads, F run) {
+    if (n_threads < 1) n_threads = 1;
+    if (n_threads > n_games / 32) n_threads = n_games / 32 > 0 ? n_games / 32 : 1;
+    if (n_threads == 1) { run(0, n_games); return; }
+    std::vector<std::thread> th;
+    const int per = (n_games + n_threads - 1) / n_threads;
+    for (int t = 0; t < n_threads; t++) {
+        const int g0 = t * per, g1 = g0 + per < n_games ? g0 + per : n_games;
+        if (g0 >= g1) break;
+        th.emplace_back(run, g0, g1);
+    }
+    for (auto &t : th) t.join();
+}
+
 }  // namespace
 
 extern "C" {
@@ -139,17 +165,18 @@ int cz_host_choose_moves(int n_games, const uint8_t *live, const int32_t *n_chil
                          int32_t *choice, double *probs, uint8_t *fallback, int n_threads) {
     if (n_games < 0 || !n_children || !ex || !mt_states || !choice || !probs || !fallback) return CZ_EINVAL;
     MT *mt = reinterpret_cast<MT *>(mt_states);
-    if (n_threads < 1) n_threads = 1;
-    if (n_threads > n_games / 32) n_threads = n_games / 32 > 0 ? n_games / 32 : 1;
-    if (n_threads == 1) { choose_range(0, n_games, live, n_children, ex, exploration, mt, choice, probs, fallback); return CZ_OK; }
-    std::vector<std::thread> th;
-    const int per = (n_games + n_threads - 1) / n_threads;
-    for (int t = 0; t < n_threads; t++) {
-        const int g0 = t * per, g1 = g0 + per < n_games ? g0 + per : n_games;
-        if (g0 >= g1) break;
-        th.emplace_back(choose_range, g0, g1, live, n_children, ex, exploration, mt, choice, probs, fallback);
-    }
-    for (auto &t : th) t.join();
+    over_games(n_games, n_threads, [=](int g0, int g1) { choose_range(g0, g1, live, n_children, ex, exploration, mt, choice, probs, fallback); });
+    return CZ_OK;
+}
+
+int cz_host_dirichlet(int n_games, const uint8_t *mask, const int32_t *n, const double *alpha_p, uint32_t *mt_states, double *eta, int n_threads) {
+    if (n_games < 0 || !n || !alpha_p || !mt_states || !eta) return CZ_EINVAL;
+    const double alpha = *alpha_p;
+    if (!(alpha > 0.0 && alpha < 1.0)) return CZ_EINVAL;
+    for (int g = 0; g < n_games; g++)
+        if ((!mask || mask[g]) && n[g] > CZ_MAXCHILD) return CZ_EINVAL;
+    MT *mt = reinterpret_cast<MT *>(mt_states);
+    over_games(n_games, n_threads, [=](int g0, int g1) { dirichlet_range(g0, g1, mask, n, alpha, mt, eta); });
     return CZ_OK;
 }
 

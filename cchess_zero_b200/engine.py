@@ -64,6 +64,7 @@ class Engine:
         self.launches = 0   # kernels of csrc/cz_engine.cu launched through this handle
         self._mate = 1 if rules == "strict" else 0          # k_root_mate after every root change of a strict engine
         self._count = torch.zeros(1, dtype=torch.int32, device="cuda:%d" % self.device)
+        self._eta = None                                      # device copy of host root-noise draws (root_noise), made on first use
 
     def close(self):
         if getattr(self, "h", None):
@@ -158,6 +159,36 @@ class Engine:
         check(lib().cz_engine_root_children(self.h, _stream(), _hp(n), _hp(mv), _hp(vis), _hp(w), _hp(p), _hp(q)),
               "cz_engine_root_children")
         return dict(n=n, moves=mv, visits=vis, w=w, p=p, q=q)
+
+    def root_counts(self):
+        """int32 [B]: the number of root children of every game (-1: root not expanded; 0: expanded without children, a mated root
+        of a strict engine).  One copy of the header lines, no kernel."""
+        n = np.zeros(self.B, dtype=np.int32)
+        check(lib().cz_engine_root_counts(self.h, _stream(), _hp(n)), "cz_engine_root_counts")
+        return n
+
+    def root_noise(self, mask, eta, eps):
+        """Root exploration noise: in every game with mask[g] that is in a search (begin_search) and has an expanded root of n > 0
+        children, root prior i becomes f32((1 - eps) * f64(P_i) + eps * eta[g, i]) (k_root_noise; no renormalisation).  eta: float64
+        [B, 128], a device tensor or a host array (copied to the device).  Expand the roots first: begin_search(0, mask) and waves
+        until unfinished() is 0."""
+        eps = float(eps)
+        if not 0.0 <= eps <= 1.0:
+            raise ValueError("root noise: eps must lie in [0, 1], not %r" % eps)
+        if isinstance(eta, torch.Tensor) and eta.is_cuda:
+            if eta.dtype != torch.float64 or tuple(eta.shape) != (self.B, MAXCHILD) or not eta.is_contiguous():
+                raise ValueError("root noise: eta must be a contiguous float64 [%d, %d] tensor" % (self.B, MAXCHILD))
+            dev = eta
+        else:
+            if self._eta is None:
+                self._eta = torch.zeros((self.B, MAXCHILD), dtype=torch.float64, device="cuda:%d" % self.device)
+            self._eta.copy_(torch.from_numpy(np.ascontiguousarray(eta, dtype=np.float64).reshape(self.B, MAXCHILD)))
+            dev = self._eta
+        m = np.ascontiguousarray(mask, dtype=np.uint8)
+        assert m.shape == (self.B,)
+        self.launches += 1
+        check(lib().cz_engine_root_noise(self.h, _stream(), _hp(m), C.c_void_p(dev.data_ptr()), C.byref(C.c_double(1.0 - eps)),
+                                         C.byref(C.c_double(eps))), "cz_engine_root_noise")
 
     def play(self, child_index, want_status=True):
         """GameBoard update + update_tree for every game with child_index >= 0; returns the status of all games (see status())

@@ -51,6 +51,22 @@ def _label_table():
     return _LABEL_OF
 
 
+def check_root_noise(root_noise):
+    """None (no root noise) or (eps, alpha) as two floats, with eps in [0, 1] and alpha in (0, 1) (AlphaZero: 0.25 and 0.3 for chess,
+    0.15 for shogi, 0.03 for Go); ValueError otherwise."""
+    if root_noise is None:
+        return None
+    try:
+        eps, alpha = (float(v) for v in root_noise)
+    except (TypeError, ValueError):
+        raise ValueError("root_noise must be None or (eps, alpha), not %r" % (root_noise,))
+    if not 0.0 <= eps <= 1.0:
+        raise ValueError("root_noise: eps must lie in [0, 1], not %r" % eps)
+    if not 0.0 < alpha < 1.0:
+        raise ValueError("root_noise: alpha must lie in (0, 1), not %r" % alpha)
+    return eps, alpha
+
+
 def sample_moves(n_children, visits, live, temperature, mt_states, exploration, n_threads=1):
     """get_action's move choice (main.py:1339-1348) for a batch of games, bit-identical to the numpy calls: pi = softmax(1/T *
     log(visits)) in float64, then RandomState.choice(p = pi) -- with exploration, p = 0.75 * pi + 0.25 * RandomState.dirichlet(0.3).
@@ -207,14 +223,17 @@ class SelfPlay:
 
     def __init__(self, n_games, forward, playouts, seeds=None, exploration=True, temperature=1,
                  nn_dtype=torch.float32, arena_words=0, auto_reset=True, device=None, keep_records=True, plan=None,
-                 plan_factory=None, lanes=1, engine=None, hashing=False, search_threads=1, compact=None, rules="reference"):
+                 plan_factory=None, lanes=1, engine=None, hashing=False, search_threads=1, compact=None, rules="reference",
+                 root_noise=None):
         """plan: an InferencePlan / NativePlan (defines the input buffer, writes logits/value in place); plan_factory(rows) builds
         one when `plan` is not given.  lanes: 1 is the only value.  rules: 'reference' or 'strict' (the search expands strictly legal
         moves only and a side without one is mated: the game ends with terminal code 3, won by the side that moved last); strict
-        rules need search_threads = 1."""
+        rules need search_threads = 1.  root_noise: None (off) or (eps, alpha): every search() first mixes Dirichlet noise into the
+        root priors of its games, P' = (1 - eps) P + eps Dir(alpha) (see search)."""
         if lanes != 1:
             raise ValueError("SelfPlay: lanes must be 1")
         self.rules = check_rules(rules, search_threads)
+        self.root_noise = check_root_noise(root_noise)
         if engine is not None and getattr(engine, "rules", "reference") != rules:
             raise ValueError("SelfPlay: the engine plays by the %r rules, not %r" % (getattr(engine, "rules", "reference"), rules))
         self.B = n_games
@@ -259,6 +278,14 @@ class SelfPlay:
         for g, sd in enumerate(seeds):
             st = np.random.RandomState(int(sd)).get_state()
             self._mt[g, :624], self._mt[g, 624] = st[1], st[2]
+        # root noise: a second stream per slot, RandomState([seed, 1]), so that the move choice draws stay those of a run without noise
+        self._noise_mt = self._eta = None                  # (and the host buffer of one search's draws, [B, 128])
+        if self.root_noise is not None:
+            self._noise_mt = np.zeros((n_games, MT_WORDS), dtype=np.uint32)
+            for g, sd in enumerate(seeds):
+                st = np.random.RandomState([int(sd), 1]).get_state()
+                self._noise_mt[g, :624], self._noise_mt[g, 624] = st[1], st[2]
+            self._eta = np.zeros((n_games, MAXCHILD), dtype=np.float64)
         self._span = [[] for _ in range(n_games)]        # the log entries of each slot's current game
         self.exploration = exploration
         self.temperature = temperature
@@ -321,14 +348,23 @@ class SelfPlay:
 
     def search(self, mask=None):
         """MCTS_tree.main for every live game (or every game with mask[g], e.g. the games where one player of a match is to move):
-        `playouts[g]` playouts each."""
+        `playouts[g]` playouts each.  With root noise, the roots are expanded and noised first (_noise_roots)."""
         m = self.live if mask is None else np.asarray(mask, dtype=bool)
         e = self.engine
         if self.plan is not None and hasattr(self.plan, "refresh_if_stale"):
             self.plan.refresh_if_stale()       # weights trained / restored since the last search (the graph reads them in place)
+        if self.root_noise is not None:
+            self._noise_roots(m)
         for p in np.unique(self.playouts[m]):
             e.begin_search(int(p), (m & (self.playouts == p)).astype(np.uint8))
         pmax = int(self.playouts[m].max()) if m.any() else 0
+        waves = self._run_waves(pmax)
+        self.waves += waves
+        return waves
+
+    def _run_waves(self, pmax, graph=True):
+        """The wave loop after begin_search, in the engine's mode: row compaction, the captured graph (graph=True) or eager waves."""
+        e = self.engine
         if self.compact:
             n = 0
 
@@ -341,17 +377,38 @@ class SelfPlay:
                 if n > 0:
                     self._eval_bucket(n)
             # done when nothing is left to evaluate and every search is complete
-            waves = run_waves(e, step, 0, pmax, evaluate, may_stop=lambda: n == 0)
-        elif self.graph is not None:
+            return run_waves(e, step, 0, pmax, evaluate, may_stop=lambda: n == 0)
+        if graph and self.graph is not None:
             def step():
                 self.graph.replay()
                 e.launches += 1          # the captured k_wave launch
-            waves = run_waves(e, step, pmax // self.K, pmax)
-        else:                            # (K leaves per game and wave in the search_threads = K schedule: pmax // K waves at least)
-            waves = run_waves(e, lambda: e.wave(self.nn_in, self.logits, self.value), pmax // self.K, pmax,
-                              evaluate=lambda: self._eval(self.nn_in))
-        self.waves += waves
-        return waves
+            return run_waves(e, step, pmax // self.K, pmax)
+        # (K leaves per game and wave in the search_threads = K schedule: pmax // K waves at least)
+        return run_waves(e, lambda: e.wave(self.nn_in, self.logits, self.value), pmax // self.K, pmax,
+                         evaluate=lambda: self._eval(self.nn_in))
+
+    def _noise_roots(self, m):
+        """Root exploration noise for the games in mask m.  A search of 0 playouts expands every pending root and runs no playout
+        (k_wave / k_wave_fifo stop at the target; a root expanded before is left alone): the network evaluates exactly the roots the
+        search itself would evaluate first.  Eager waves, not the captured graph, so that no network pass runs without a leaf.  Then,
+        for every searched, live game with n >= 1 root children, in slot order: eta = RandomState([seed, 1]).dirichlet(alpha * ones(n))
+        (cz_host_dirichlet) and P' = f32((1 - eps) f64(P) + eps eta) on the device (k_root_noise).  The noised root block is dropped
+        by the next play (only the chosen subtree is kept), so games at rest never hold noised priors."""
+        import ctypes as C
+        from ._lib import lib
+        e = self.engine
+        e.begin_search(0, m.astype(np.uint8))
+        self.waves += self._run_waves(0, graph=False)
+        n = np.ascontiguousarray(e.root_counts(), dtype=np.int32)
+        sel = (m & self.live & (n > 0)).astype(np.uint8)
+        if not sel.any():
+            return
+        eps, alpha = self.root_noise
+        vp = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
+        rc = lib().cz_host_dirichlet(self.B, vp(sel), vp(n), C.byref(C.c_double(alpha)), vp(self._noise_mt), vp(self._eta), self._threads)
+        if rc:
+            raise EngineError("cz_host_dirichlet failed (%d)" % rc)
+        e.root_noise(sel, self._eta, eps)
 
     # -- one ply for every live game ------------------------------------------------------------
     def step(self):
@@ -420,9 +477,9 @@ class SelfPlay:
 
     def save_games(self, path):
         """Every game in flight into one np.savez file (written to a temporary file, then renamed): the engine's trees and game state
-        (Engine.snapshot) and the host state -- boards, sides, live, the per-slot MT19937 states, plies, temperature and each slot's
-        unfinished record (its players and log span).  load_games continues exactly where this left off.  The finished games must
-        have been handed over with pop_finished first."""
+        (Engine.snapshot) and the host state -- boards, sides, live, the per-slot MT19937 states (and, with root noise, the noise
+        streams' states under 'noise_mt'), plies, temperature and each slot's unfinished record (its players and log span).  load_games
+        continues exactly where this left off.  The finished games must have been handed over with pop_finished first."""
         if self.finished:
             raise ValueError("save_games: %d finished games were not drained with pop_finished()" % len(self.finished))
         from .train import _savez
@@ -430,14 +487,16 @@ class SelfPlay:
         rows = [(lg, g) for g in range(self.B) for lg in self._span[g]]
         log = {"log_" + k: np.asarray([lg[k][g] for lg, g in rows], dtype=dt).reshape((len(rows),) + shp) for k, shp, dt in self._LOG}
         players = [self.records[g].players for g in range(self.B)]
+        if self.root_noise is not None:
+            log["noise_mt"] = self._noise_mt
         _savez(path, engine=blob, boards=self.boards, sides=self.sides, live=self.live, mt=self._mt, plies=np.int64(self.plies),
                temperature=np.asarray(self.temperature, dtype=np.float64), span_len=np.asarray([len(s) for s in self._span], dtype=np.int64),
                players_len=np.asarray([len(p) for p in players], dtype=np.int64),
                players=np.asarray([p for ps in players for p in ps], dtype=np.uint8), **log)
 
     def load_games(self, path):
-        """Restore what save_games wrote into this SelfPlay (same number of games and engine kind; the engine is restored in place, so
-        a captured graph stays valid).  The file is read without pickle and checked; ValueError / EngineError leave everything as it
+        """Restore what save_games wrote into this SelfPlay (same number of games and engine kind, root noise on in both or in neither;
+        the engine is restored in place, so a captured graph stays valid).  The file is read without pickle and checked; ValueError / EngineError leave everything as it
         was."""
         with np.load(path, allow_pickle=False) as d:
             a = {k: d[k] for k in d.files}
@@ -448,6 +507,11 @@ class SelfPlay:
         rows = int(a["span_len"].sum()) if "span_len" in a else -1
         for k, shp, dt in self._LOG:
             want["log_" + k] = ((rows,) + shp, dt)
+        if ("noise_mt" in a) != (self.root_noise is not None):        # the noise streams are part of an exact resume
+            raise ValueError("games file: saved %s root noise, this SelfPlay runs %s" % (("with", "without") if "noise_mt" in a
+                                                                                        else ("without", "with")))
+        if self.root_noise is not None:
+            want["noise_mt"] = ((B, MT_WORDS), np.uint32)
         for k, (shp, dt) in want.items():
             if k not in a or a[k].dtype != dt or (shp is not None and a[k].shape != shp):
                 raise ValueError("games file: '%s' missing or not %s %s" % (k, np.dtype(dt).name, shp))
@@ -479,6 +543,8 @@ class SelfPlay:
             self.records[g].players = [int(p) for p in a["players"][ends[g] - a["players_len"][g]:ends[g]]]
         self.boards, self.sides, self.live = a["boards"].copy(), a["sides"].copy(), a["live"].copy()
         self._mt[:] = a["mt"]
+        if self.root_noise is not None:
+            self._noise_mt[:] = a["noise_mt"]
         self.plies = int(a["plies"])
 
     def play_games(self, max_plies=100000):

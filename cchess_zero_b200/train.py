@@ -279,21 +279,24 @@ class Trainer:
     reference does no augmentation).
 
     save(dir) / load(dir) keep everything a run needs to continue: the network(s) with their optimizer state, the replay buffer,
-    the sampler's random state, every game slot's MT19937 state, lr_multiplier, the counters and the games in flight
-    (SelfPlay.save_games: the engine's trees and each slot's unfinished record), so a resumed run plays on exactly as the
-    uninterrupted one.  A directory saved without games.npz resumes with fresh games in every slot (drawing from the restored
+    the sampler's random state, every game slot's MT19937 states (move choice and, with root noise, the noise stream), lr_multiplier,
+    the counters and the games in flight (SelfPlay.save_games: the engine's trees and each slot's unfinished record), so a resumed
+    run plays on exactly as the uninterrupted one.  load refuses a run saved with other rules or another root noise setting.  A directory saved without games.npz resumes with fresh games in every slot (drawing from the restored
     per-slot streams)."""
 
     def __init__(self, network, n_games, playouts, search_threads=1, batch_size=512, buffer_size=10000, epochs=5, kl_targ=0.025,
                  learning_rate=1e-3, updates_per_game=1, mirror=False, eval_every=0, eval_games=10, eval_playouts=None,
-                 gate_threshold=0.55, checkpoint_every=100, seed=0, arena_words=1 << 20, best=None, rules="reference"):
+                 gate_threshold=0.55, checkpoint_every=100, seed=0, arena_words=1 << 20, best=None, rules="reference", root_noise=None):
         """rules: 'reference' or 'strict' -- self-play and the gate's matches search strictly legal moves only and a side without
-        one is mated (the network learns the full rules of xiangqi); strict rules need search_threads = 1."""
+        one is mated (the network learns the full rules of xiangqi); strict rules need search_threads = 1.  root_noise: None or
+        (eps, alpha) -- Dirichlet noise on the root priors of every self-play search (SelfPlay root_noise); the gate's matches
+        stay noise-free."""
         from .engine import check_rules
-        from .selfplay import network_selfplay
+        from .selfplay import check_root_noise, network_selfplay
         if eval_every and (eval_games <= 0 or eval_games % 2):
             raise ValueError("eval_games must be a positive even number (colour-swapped pairs)")
         self.rules = check_rules(rules, search_threads)
+        self.root_noise = check_root_noise(root_noise)
         self.network = network
         self.n_games, self.playouts, self.search_threads = int(n_games), playouts, int(search_threads)
         self.batch_size, self.epochs, self.kl_targ = int(batch_size), int(epochs), kl_targ
@@ -310,7 +313,7 @@ class Trainer:
         self.buffer = ReplayBuffer(buffer_size, network.device.index)
         self.sp = network_selfplay(self.best or network, self.n_games, playouts, seeds=[self.seed * self.n_games + g for g in range(self.n_games)],
                                    search_threads=self.search_threads, arena_words=arena_words, auto_reset=True, keep_records=True,
-                                   rules=self.rules)
+                                   rules=self.rules, root_noise=self.root_noise)
         self.sp.capture_graph()
         self.games = self.positions = self.updates = self.train_steps = self.promotions = self.gates = self.plies = 0
         self.next_gate = self.eval_every
@@ -435,8 +438,12 @@ class Trainer:
             _save_network(self.best, os.path.join(directory, "best"))
         self.buffer.save(os.path.join(directory, "replay.npz"))
         version, internal, gauss = self.rng.getstate()
+        # root_noise: [eps, alpha], or empty when off; the noise streams' states go with it
+        noise = dict(root_noise=np.asarray(self.root_noise or (), dtype=np.float64))
+        if self.root_noise is not None:
+            noise["noise_mt"] = self.sp._noise_mt
         _savez(os.path.join(directory, "trainer.npz"), rng_version=version, rng_internal=np.asarray(internal, dtype=np.uint32),
-               rng_gauss=np.float64(0.0 if gauss is None else gauss), rng_has_gauss=gauss is not None, mt=self.sp._mt,
+               rng_gauss=np.float64(0.0 if gauss is None else gauss), rng_has_gauss=gauss is not None, mt=self.sp._mt, **noise,
                lr_multiplier=self.lr_multiplier, next_gate=self.next_gate, rules=np.asarray(self.rules),
                counters=np.asarray([self.games, self.positions, self.updates, self.train_steps, self.promotions, self.gates, self.plies],
                                    dtype=np.int64))
@@ -450,6 +457,11 @@ class Trainer:
             saved = str(d["rules"]) if "rules" in d.files else "reference"          # (runs saved before the rules choice existed)
             if saved != self.rules:
                 raise ValueError("saved run plays by the %r rules, this Trainer by %r" % (saved, self.rules))
+            rn = d["root_noise"] if "root_noise" in d.files else np.zeros(0)    # (runs saved before root noise existed: off)
+            saved = tuple(float(v) for v in rn) if rn.size else None
+            if saved != self.root_noise:
+                raise ValueError("saved run has root noise %r, this Trainer %r" % (saved, self.root_noise))
+            noise_mt = d["noise_mt"].copy() if self.root_noise is not None else None
             gauss = float(d["rng_gauss"]) if bool(d["rng_has_gauss"]) else None
             self.rng.setstate((int(d["rng_version"]), tuple(int(v) for v in d["rng_internal"]), gauss))
             mt = d["mt"].copy()
@@ -464,14 +476,17 @@ class Trainer:
         if os.path.isfile(games):
             self.sp.load_games(games)
         else:
-            self._restart_games(mt)
+            self._restart_games(mt, noise_mt)
 
-    def _restart_games(self, mt):
-        """Every slot starts a fresh game from the start position, drawing its moves from the stream mt[slot]."""
+    def _restart_games(self, mt, noise_mt=None):
+        """Every slot starts a fresh game from the start position, drawing its moves from the stream mt[slot] (and its root noise
+        from noise_mt[slot])."""
         from .selfplay import GameRecord
         sp = self.sp
         sp.engine.reset()
         sp._mt[:] = mt
+        if noise_mt is not None:
+            sp._noise_mt[:] = noise_mt
         sp._span = [[] for _ in range(sp.B)]
         sp.records = [GameRecord(g, None, sp.temperature) for g in range(sp.B)]
         sp.boards = np.tile(sp._start_board, (sp.B, 1))
@@ -506,6 +521,8 @@ def main(argv=None):
     ap.add_argument("--resume", action="store_true", help="continue the run saved in --save-dir")
     ap.add_argument("--rules", choices=("reference", "strict"), default="reference",
                     help="strict: search strictly legal moves only; a side without one is mated (needs --search-threads 1)")
+    ap.add_argument("--root-noise", nargs=2, type=float, metavar=("EPS", "ALPHA"), default=None,
+                    help="Dirichlet noise on the self-play root priors: P' = (1 - EPS) P + EPS Dir(ALPHA), e.g. 0.25 0.3")
     a = ap.parse_args(argv)
     from .net import policy_value_network
     out = sys.stdout
@@ -516,7 +533,7 @@ def main(argv=None):
         t = Trainer(net, a.games, a.playouts, search_threads=a.search_threads, batch_size=a.batch_size, buffer_size=a.buffer_size,
                     epochs=a.epochs, learning_rate=a.learning_rate, updates_per_game=a.updates_per_game, mirror=a.mirror,
                     eval_every=a.eval_every, eval_games=a.eval_games, eval_playouts=a.eval_playouts, gate_threshold=a.gate_threshold,
-                    checkpoint_every=a.checkpoint_every, seed=a.seed, rules=a.rules)
+                    checkpoint_every=a.checkpoint_every, seed=a.seed, rules=a.rules, root_noise=a.root_noise)
         if t.best is not None:
             t.best.save_dir = os.path.join(a.save_dir, "best")
         if a.resume and os.path.isfile(os.path.join(a.save_dir, "trainer.npz")):

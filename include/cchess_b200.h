@@ -210,6 +210,17 @@ int cz_engine_unfinished_async(cz_engine *e, void *stream, int32_t *dev_count);
 int cz_engine_root_children(cz_engine *e, void *stream, int32_t *n_children /* [B] (-1: root not expanded) */,
                             uint16_t *moves /* [B][128] */, int32_t *visits /* [B][128] */,
                             float *w /* [B][128] */, float *p /* [B][128] */, float *q /* [B][128] */);
+/* The root's child count of every game (-1: root not expanded, 0: expanded without children) into HOST counts [B]: one copy of
+ * the header lines, synchronises stream. */
+int cz_engine_root_counts(cz_engine *e, void *stream, int32_t *counts /* [B] */);
+/* Root exploration noise (AlphaZero: P' = (1 - eps) P + eps eta, once per move search; the reference's root Dirichlet is a no-op):
+ * for every game with mask[g] != 0 (HOST mask, NULL = all), active (cz_engine_begin_search) and with an expanded root of n > 0
+ * children, root prior i becomes f32(keep * f64(P_i) + eps * eta[g][i]) (separately rounded f64 products and sum, no FMA; no
+ * renormalisation).  eta: DEVICE f64 [B][128]; *keep is 1 - *eps as the caller computed it, both in [0, 1] (else CZ_EINVAL).  Expand
+ * the roots first: cz_engine_begin_search(playouts = 0) and waves until cz_engine_unfinished is 0 expand every pending root and run
+ * no playout.  Nothing else in the tree changes; cz_engine_play drops the noised block with the rest of the old root. */
+int cz_engine_root_noise(cz_engine *e, void *stream, const uint8_t *mask, const double *eta, const double *keep /* host [1] */,
+                         const double *eps /* host [1] */);
 
 /* Play child_index[g] (index into the root's children; < 0 = leave game g alone):
  * GameBoard state update (main.py:1522-1528) + MCTS_tree.update_tree (272-276): the chosen child's
@@ -307,6 +318,12 @@ int cz_net_heads(const void *x, int B, const float *wh, const float *bh, const f
 int cz_host_choose_moves(int n_games, const uint8_t *live, const int32_t *n_children, const double *ex /* [B][128] */, int exploration,
                          uint32_t *mt_states /* [B][626] */, int32_t *choice /* [B] */, double *probs /* [B][128] */, uint8_t *fallback /* [B] */,
                          int n_threads);
+/* Root exploration noise, host side: for every game g with mask[g] != 0 (mask NULL = all) and n[g] > 0, eta[g][:n[g]] =
+ * RandomState.dirichlet(alpha * ones(n[g])) drawn from mt_states[g] (layout as above), bit-identical to numpy, the state advanced
+ * exactly as numpy advances it.  Other games: neither their state nor their eta row is touched.  0 < *alpha < 1 (the shape-below-1
+ * branch of numpy's legacy gamma) and n[g] <= 128 for every selected game, else CZ_EINVAL before any draw.  HOST memory only. */
+int cz_host_dirichlet(int n_games, const uint8_t *mask, const int32_t *n /* [B] */, const double *alpha /* host [1] */, uint32_t *mt_states /* [B][626] */,
+                      double *eta /* [B][128] */, int n_threads);
 
 /* cz_net_heads for large batches: policy FC on wgmma (operands bulk-copied in the K-major no-swizzle layout), 1x1 head convolution on
  * mma.sync, value MLP concurrently.  wp_tiled: dev fp16 [17 label tiles][24 k-chunks][128 labels][8 features] (labels >= 2086 zero),
