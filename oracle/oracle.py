@@ -225,23 +225,36 @@ def flip_label(m):
     return "".join(str(9 - int(a)) if a.isdigit() else a for a in m)
 
 
-def selfplay_game(net, playouts, rs, exploration=True, temperature=1, max_plies=10000, search_threads=1):
+def game_end(board, side, rr):
+    """The reference's end test after a move (main.py:1380-1392, in the engine's order): a king taken -> (1, winner), rr >= 60 ->
+    (2, -1); (0, -1) while the game runs."""
+    hasK, hask = (board == 1).any(), (board == 8).any()
+    if not hasK or not hask:
+        return 1, (1 if not hasK else 0) if hask else 0
+    return (2, -1) if rr >= 60 else (0, -1)
+
+
+def selfplay_game(net, playouts, rs, exploration=True, temperature=1, max_plies=10000, search_threads=1, tree=None, search=None,
+                  end=game_end):
     """cchess_main.selfplay (main.py:1493-1554) + get_action (1332-1358) over the C tree.
 
     rs: np.random.RandomState standing in for the global np.random of the reference.
     search_threads > 1: every search runs the reference's K-coroutine schedule in canonical form (co_tree_search_fifo).
-    Returns dict(states, pis (dense [n,2086] f64), z, actions, visits).
+    tree, search, end: another specification's tree at the start position, its search(side, rr) -> error and its end test
+    end(board, side, rr) -> (code, winner) (tests/search_spec.py: strict rules, root noise) instead of this module's.
+    Returns dict(states, pis (dense [n,2086] f64), z, actions, visits, end (the end code), boards (every position played from), players).
     """
-    lab = labels()
-    l2i = {m: i for i, m in enumerate(lab)}
-    tree = Tree()
+    if tree is None:
+        tree = Tree()
+        search = (lambda side, rr: tree.search(side, rr, playouts, net)) if search_threads <= 1 else \
+            (lambda side, rr: tree.search_fifo(side, rr, playouts, search_threads, net))
+    l2i = {m: i for i, m in enumerate(labels())}
     board = from_state(START)
     side, rr = 0, 0
-    states, pis, players, actions, all_visits = [], [], [], [], []
-    z = None
+    states, pis, players, actions, all_visits, boards = [], [], [], [], [], []
     with np.errstate(divide="ignore"):
         while True:
-            err = tree.search(side, rr, playouts, net) if search_threads <= 1 else tree.search_fifo(side, rr, playouts, search_threads, net)
+            err = search(side, rr)
             if err:
                 raise RuntimeError("oracle tree error %d" % err)
             mv, N, W, P, Q = tree.root_children()
@@ -255,6 +268,7 @@ def selfplay_game(net, playouts, rs, exploration=True, temperature=1, max_plies=
             act = rs.choice(acts, p=p)
             idx = acts.index(act)
             tree.update(idx)
+            boards.append(board.copy())
             sboard = flip_board(board) if side == 1 else board
             states.append(to_state(sboard))
             prob = np.zeros(NLABEL)
@@ -267,14 +281,11 @@ def selfplay_game(net, playouts, rs, exploration=True, temperature=1, max_plies=
             board, cap = apply_move(board, mv[idx])
             side ^= 1
             rr = rr + 1 if cap == 0 else 0
-            hasK, hask = (board == 1).any(), (board == 8).any()
-            if not hasK or not hask:
-                winner = 1 if not hasK else 0
-                if not hask:
-                    winner = 0
+            code, winner = end(board, side, rr)
+            if code in (1, 3):
                 z = np.where(np.array(players) == winner, 1.0, -1.0)
                 break
-            if rr >= 60 or len(states) >= max_plies:
+            if code == 2 or len(states) >= max_plies:
                 z = np.zeros(len(players))
                 break
-    return dict(states=states, pis=np.array(pis), z=z, actions=actions, visits=all_visits)
+    return dict(states=states, pis=np.array(pis), z=z, actions=actions, visits=all_visits, end=code, boards=boards, players=players)

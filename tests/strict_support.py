@@ -1,5 +1,5 @@
 """TEST INFRASTRUCTURE shared by test_strict_host.py and test_gpu_strict.py: the brute-force strict-legality oracle
-(tests/strict_oracle.c, compiled together with oracle/cchess_oracle.c), the host build of the product's own per-lane source
+(tests/strict_oracle.c, built into one library with the search specification), the host build of the product's own per-lane source
 (tests/host_strict_harness.cu), seeded position generators and hand-made positions with known answers."""
 import ctypes as C
 import os
@@ -26,14 +26,32 @@ def _p(a):
 
 
 def oracle_lib():
+    """The test specification library, built once per session: tests/strict_search_oracle.c (which includes oracle/cchess_oracle.c)
+    and tests/strict_oracle.c; search_spec.py wraps its trees."""
     if "so" not in _libs:
-        so = os.path.join(_dir(), "libstrictoracle.so")
+        so = os.path.join(_dir(), "libsearchspec.so")
         subprocess.check_call([os.environ.get("CC", "gcc"), "-O2", "-fPIC", "-ffp-contract=off", "-shared", "-o", so,
-                               os.path.join(ROOT, "tests", "strict_oracle.c"), os.path.join(ROOT, "oracle", "cchess_oracle.c"), "-lm", "-lpthread"])
+                               os.path.join(ROOT, "tests", "strict_search_oracle.c"), os.path.join(ROOT, "tests", "strict_oracle.c"),
+                               "-lm", "-lpthread"])
         L = C.CDLL(so)
-        L.so_strict_moves_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 4
-        L.so_random_play.argtypes = [C.c_uint64, C.c_int, C.c_void_p, C.c_void_p]
-        L.so_random_setup.argtypes = [C.c_uint64, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+        vp, i32 = C.c_void_p, C.c_int
+        L.so_strict_moves_batch.argtypes = [vp, vp, i32] + [vp] * 4
+        L.so_random_play.argtypes = [C.c_uint64, i32, vp, vp]
+        L.so_random_setup.argtypes = [C.c_uint64, i32, i32, i32, vp, vp]
+        L.so_in_check.argtypes = [vp, i32]
+        L.so_strict_moves.argtypes = [vp, i32, vp, vp]
+        L.co_tree_new.restype = L.ss_tree_new.restype = vp
+        L.co_tree_new.argtypes = L.ss_tree_new.argtypes = [vp]
+        L.co_tree_free.argtypes = [vp]
+        L.co_tree_search_fake.argtypes = L.ss_tree_search_fake.argtypes = [vp, i32, i32, i32, i32]
+        L.co_tree_search_fifo.argtypes = [vp, i32, i32, i32, i32, i32]
+        L.co_tree_root_children.argtypes = [vp] * 6
+        L.co_tree_update.argtypes = [vp, i32]
+        L.rn_set_root_P.argtypes = [vp, vp]
+        L.ss_tree_root_mated.argtypes = [vp]
+        L.co_tree_stats.argtypes = L.ss_tree_stats.argtypes = [vp, vp]
+        L.co_tree_signature.argtypes = L.ss_tree_signature.argtypes = [vp, vp, C.c_long]
+        L.co_tree_signature.restype = L.ss_tree_signature.restype = C.c_long
         _libs["so"] = L
     return _libs["so"]
 

@@ -1,4 +1,4 @@
-"""CPU tier of the arena: match statistics (score, Elo, interval, gate), argument checks and the match oracle itself."""
+"""CPU tier of the arena: match statistics (score, Elo, interval, gate), argument checks and the match specification itself."""
 import math
 
 import numpy as np
@@ -58,7 +58,7 @@ def test_match_rejects_odd_or_empty_game_counts(n):
 
 
 def test_match_oracle_is_deterministic_and_legal():
-    from arena_oracle import match_game
+    from search_spec import match_game
     from oracle import oracle as O
     a = match_game("hash_signed", "mod17", 12, np.random.RandomState(3), 6, 1.0, 1e-3, max_plies=24, signatures=True)
     b = match_game("hash_signed", "mod17", 12, np.random.RandomState(3), 6, 1.0, 1e-3, max_plies=24, signatures=True)

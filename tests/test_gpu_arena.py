@@ -1,5 +1,5 @@
 """Arena on the device: Engine.play_moves (cz_engine_play_moves) and arena.Match, checked against Engine.play, the rules kernels and
-the C oracle (tests/arena_oracle.py)."""
+the C oracle (tests/search_spec.py)."""
 import contextlib
 import io
 
@@ -200,7 +200,7 @@ def test_play_moves_in_a_finished_game_is_illegal_and_no_move_is_silent():
 
 @pytest.mark.parametrize("K", [1, 16])
 def test_match_equals_oracle(K):
-    from arena_oracle import match_game
+    from search_spec import match_game
     from cchess_zero_b200.arena import Match
     from cchess_zero_b200.fakenet import FakeNet
     n, P, T0, plies0, cap = 8, 60, 1.0, 6, 80

@@ -1,6 +1,6 @@
 """Root exploration noise on the device (SelfPlay(root_noise=(eps, alpha)): a root-expansion pre-pass, cz_host_dirichlet and
 k_root_noise): the kernel against the formula word for word, the pre-pass's transparency at eps = 0, whole self-play games against the
-specification trees (tests/root_noise_support.py) under both rules and both search schedules, and exact resumes.  Bit-exact everywhere."""
+specification trees (tests/search_spec.py) under both rules and both search schedules, and exact resumes.  Bit-exact everywhere."""
 import contextlib
 import io
 import os
@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 import torch
 
-import root_noise_support as R
+import search_spec as S
 
 pytestmark = pytest.mark.gpu
 
@@ -79,7 +79,7 @@ def test_kernel_equals_the_formula_and_changes_nothing_else(kind):
     p = e.root_children(want_wpq=True)["p"]
     for g in range(B):
         k = max(int(n[g]), 0)                              # (-1: a root that was not searched and is not expanded)
-        want = R.mix(rc["p"][g, :k], eta[g, :k], eps) if mask[g] else rc["p"][g, :k]
+        want = S.mix(rc["p"][g, :k], eta[g, :k], eps) if mask[g] else rc["p"][g, :k]
         assert np.array_equal(p[g, :k].view(np.uint32), want.view(np.uint32)), g
         sig = e.tree_signature(g)
         roots = _root_records(sig)
@@ -149,7 +149,9 @@ def test_noisy_selfplay_games_equal_the_specification(kind):
     assert len(out) == B
     for slot, rec in out:
         with np.errstate(all="ignore"):
-            r = R.selfplay_game(kind, net, P, seeds[slot], eps, alpha)
+            r = S.selfplay_game(net, P, np.random.RandomState(seeds[slot]), rules="strict" if kind == "strict" else "reference",
+                                search_threads=16 if kind == "fifo" else 1,
+                                root_noise=(eps, alpha, np.random.RandomState([seeds[slot], 1])))
         assert rec.states == r["states"] and rec.actions == r["actions"], slot
         assert [tuple(int(v) for v in x) for x in rec.visits] == r["visits"], slot
         assert np.array_equal(rec.z, r["z"]) and np.array_equal(rec.dense_pi(), r["pis"]), slot

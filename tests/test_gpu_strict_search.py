@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 import torch
 
-import strict_search_support as S
+import search_spec as S
 from strict_support import oracle_strict
 
 pytestmark = pytest.mark.gpu
@@ -62,7 +62,7 @@ def test_trees_equal_the_specification():
     tot = dict(n_expand=0, n_playout=0, sum_L=0, sum_c=0, sum_C=0)
     mated_leaves = in_check = 0
     for g, c in enumerate(cases):
-        t = S.StrictTree(c["board"])
+        t = S.Tree(c["board"], "strict")
         assert t.search(c["side"], c["rr"], c["playouts"], c["net"]) == 0
         sig = t.signature()
         assert np.array_equal(sig, e.tree_signature(g)), g
@@ -89,7 +89,7 @@ def test_selfplay_games_equal_the_specification(net, O):
     ends = []
     for slot, rec in out:
         with np.errstate(all="ignore"):
-            r = S.selfplay_game(net, P, np.random.RandomState(seeds[slot]))
+            r = S.selfplay_game(net, P, np.random.RandomState(seeds[slot]), rules="strict")
         assert rec.states == r["states"] and rec.actions == r["actions"], slot
         assert np.array_equal(rec.z, r["z"]) and np.array_equal(rec.dense_pi(), r["pis"]), slot
         ends.append(r["end"])
@@ -156,7 +156,7 @@ def test_strict_match_equals_the_specification():
         o = g % (n // 2) % 2
         with np.errstate(all="ignore"):
             x = S.match_game(red, black, P, np.random.RandomState(g), plies0, T0, 1e-3, board=openings[0][o], side=int(openings[1][o]),
-                             rr=int(openings[2][o]), max_plies=cap)
+                             rr=int(openings[2][o]), max_plies=cap, rules="strict")
         rec = r.games[g]
         assert rec["moves"] == x["moves"] and rec["winner"] == "wbt"[x["winner"]] and rec["plies"] == x["plies"], g
     # strict openings: every move drawn is strictly legal and the position reached is a running game

@@ -11,6 +11,8 @@ import numpy as np
 import pytest
 import torch
 
+from search_spec import StandIn
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
@@ -308,76 +310,6 @@ def test_replay_persistence_round_trip_and_rng_resume(tmp_path):
     assert np.array_equal(np.random.rand(3), expect_np) and random.random() == expect_py
 
 
-class _OracleEngine:
-    """Engine-interface stand-in over the CPU oracle trees: lets the CPU suite run SelfPlay's HOST logic (visit counts -> pi,
-    RNG draws, tuple recording, game end / reset handling) end to end.  Test infrastructure only."""
-    torch_device = "cpu"
-
-    def __init__(self, n, net):
-        from oracle import oracle as O
-        self.O, self.B, self.net, self.device, self.launches = O, n, net, 0, 0
-        self.trees = [O.Tree() for _ in range(n)]
-        self.boards = np.tile(O.from_state(O.START), (n, 1))
-        self.side = np.zeros(n, np.uint8); self.rr = np.zeros(n, np.int32); self.ply = np.zeros(n, np.int32)
-        self.terminal = np.zeros(n, np.uint8); self.winner = -np.ones(n, np.int8)
-        self.target = np.zeros(n, np.int64); self.pending_search = np.zeros(n, bool)
-
-    def reset(self, mask=None, boards=None, sides=None, rr=None):
-        for g in range(self.B):
-            if mask is None or mask[g]:
-                self.trees[g].reload(); self.boards[g] = self.O.from_state(self.O.START)
-                self.side[g] = 0; self.rr[g] = 0; self.ply[g] = 0; self.terminal[g] = 0; self.winner[g] = -1
-
-    def begin_search(self, playouts, mask=None):
-        for g in range(self.B):
-            if (mask[g] if mask is not None else not self.terminal[g]):
-                self.target[g] = playouts; self.pending_search[g] = True
-
-    def wave(self, nn_in, logits, value):       # the whole search of every selected game happens in the first "wave"
-        for g in np.nonzero(self.pending_search)[0]:
-            assert self.trees[g].search(int(self.side[g]), int(self.rr[g]), int(self.target[g]), self.net) == 0
-        self.pending_search[:] = False
-
-    def unfinished(self):
-        return int(self.pending_search.sum())
-
-    def root_children(self, want_wpq=True):
-        n = np.zeros(self.B, np.int32); mv = np.zeros((self.B, 128), np.uint16); vis = np.zeros((self.B, 128), np.int32)
-        w = np.zeros((self.B, 128), np.float32); p = np.zeros((self.B, 128), np.float32); q = np.zeros((self.B, 128), np.float32)
-        for g, t in enumerate(self.trees):
-            m, N, W, P, Q = t.root_children()
-            k = len(m); n[g] = k; mv[g, :k] = m; vis[g, :k] = N; w[g, :k] = W; p[g, :k] = P; q[g, :k] = Q
-        return dict(n=n, moves=mv, visits=vis, w=w, p=p, q=q)
-
-    def play(self, choice, want_status=True):
-        q = np.zeros(self.B, np.float32)
-        for g, c in enumerate(choice):
-            if c < 0:
-                continue
-            rc = self.trees[g].root_children()
-            m = rc[0][c]
-            q[g] = rc[4][c]
-            self.trees[g].update(int(c))
-            self.boards[g], cap = self.O.apply_move(self.boards[g], int(m))
-            self.side[g] ^= 1; self.rr[g] = self.rr[g] + 1 if cap == 0 else 0; self.ply[g] += 1
-            if cap == 1: self.terminal[g], self.winner[g] = 1, 1
-            elif cap == 8: self.terminal[g], self.winner[g] = 1, 0
-            elif self.rr[g] >= 60: self.terminal[g] = 2
-        st = self.status()
-        st["q"] = q
-        return st if want_status else None
-
-    def status(self, boards=True):
-        return dict(terminal=self.terminal.copy(), winner=self.winner.copy(), ply=self.ply.copy(), rr=self.rr.copy(),
-                    side=self.side.copy(), boards=self.boards.copy())
-
-    def counters(self):
-        return dict(error=0)
-
-    def raise_on_error(self):
-        return self.counters()
-
-
 def test_selfplay_host_loop_on_cpu_stand_in_engine_matches_reference_vectors():
     """SelfPlay.step's host side (softmax(log N), Dirichlet mix, choice, tuple recording, z, game end) against the reference's
     own self-play tuples, with the device engine replaced by the oracle trees."""
@@ -387,7 +319,7 @@ def test_selfplay_host_loop_on_cpu_stand_in_engine_matches_reference_vectors():
     from cchess_zero_b200.selfplay import SelfPlay
     import hashlib
     games = [g for g in load_golden("selfplay.json")["games"] if g["net"] == "hash_pos"]
-    eng = _OracleEngine(len(games), "hash_pos")
+    eng = StandIn(len(games), "hash_pos")
     sp = SelfPlay(len(games), lambda x: None, [g["playouts"] for g in games], seeds=[g["seed"] for g in games], auto_reset=False, engine=eng)
     with np.errstate(all="ignore"):
         out = sp.play_games()
@@ -432,7 +364,7 @@ def test_selfplay_auto_reset_path_on_cpu_stand_in_engine():
     game must equal what the oracle plays with the same slot RNG stream continued across games."""
     from cchess_zero_b200.selfplay import SelfPlay
     B, P, net = 6, 8, "hash_pos"
-    eng = _OracleEngine(B, net)
+    eng = StandIn(B, net)
     sp = SelfPlay(B, lambda x: None, P, seeds=[40 + i for i in range(B)], auto_reset=True, engine=eng)
     with np.errstate(all="ignore"):
         for _ in range(260):

@@ -6,7 +6,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import root_noise_support as R
+import search_spec as S
 
 MT_WORDS = 626
 
@@ -105,7 +105,7 @@ def test_root_noise_argument_is_validated():
         with pytest.raises(ValueError, match="root_noise must be"):
             check_root_noise(bad)
     with pytest.raises(ValueError, match="alpha"):
-        SelfPlay(2, lambda x: None, 8, engine=R.StandIn(2, "hash_pos"), root_noise=(0.25, 1.5))
+        SelfPlay(2, lambda x: None, 8, engine=S.StandIn(2, "hash_pos"), root_noise=(0.25, 1.5))
     with pytest.raises(ValueError, match="eps"):
         Trainer(None, 2, 8, root_noise=(2.0, 0.3))
 
@@ -114,7 +114,7 @@ def test_search_draws_in_slot_order_for_searched_live_games_with_children():
     from cchess_zero_b200.selfplay import SelfPlay
     B, eps, alpha = 6, 0.25, 0.3
     seeds = [40 + 7 * g for g in range(B)]
-    e = R.StandIn(B, "hash_pos")
+    e = S.StandIn(B, "hash_pos")
     sp = SelfPlay(B, lambda x: None, 16, seeds=seeds, engine=e, root_noise=(eps, alpha))
     rn = [np.random.RandomState([s, 1]) for s in seeds]
     sp.live[4] = False                                      # a game that is not running
@@ -147,24 +147,21 @@ def test_search_draws_in_slot_order_for_searched_live_games_with_children():
     assert [c[0] for c in e.log] == ["begin_search", "root_counts"]
 
 
-@pytest.mark.parametrize("kind", ["reference", "strict"])
-def test_selfplay_host_loop_with_noise_equals_the_specification(kind):
+@pytest.mark.parametrize("rules", ["reference", "strict"])
+def test_selfplay_host_loop_with_noise_equals_the_specification(rules):
     from cchess_zero_b200.selfplay import SelfPlay
     B, P, net, eps, alpha = 3, 16, "hash_signed", 0.25, 0.3
     seeds = [900 + 11 * g for g in range(B)]
-    sp = SelfPlay(B, lambda x: None, P, seeds=seeds, auto_reset=False, engine=R.StandIn(B, net, kind), rules=sp_rules(kind),
+    sp = SelfPlay(B, lambda x: None, P, seeds=seeds, auto_reset=False, engine=S.StandIn(B, net, rules), rules=rules,
                   root_noise=(eps, alpha))
     with np.errstate(all="ignore"):
         out = sp.play_games(max_plies=120)
     for slot, rec in out:
         with np.errstate(all="ignore"):
-            r = R.selfplay_game(kind, net, P, seeds[slot], eps, alpha)
+            r = S.selfplay_game(net, P, np.random.RandomState(seeds[slot]), rules=rules,
+                                root_noise=(eps, alpha, np.random.RandomState([seeds[slot], 1])))
         assert rec.states == r["states"] and rec.actions == r["actions"], slot
         assert np.array_equal(rec.z, r["z"]) and np.array_equal(rec.dense_pi(), r["pis"]), slot
-
-
-def sp_rules(kind):
-    return "strict" if kind == "strict" else "reference"
 
 
 def test_noise_changes_the_search_below_a_visited_root():
@@ -172,17 +169,17 @@ def test_noise_changes_the_search_below_a_visited_root():
     the tree's root N never grows during a search, so at a fresh root N = 0, U = 0 and the priors do not steer its children)."""
     from oracle import oracle as O
     b = O.from_state(O.START)
-    plain, noisy = R.Tree("reference", b), R.Tree("reference", b)
+    plain, noisy = S.Tree(b), S.Tree(b)
     for t in (plain, noisy):
         assert t.search(0, 0, 200, "hash_pos") == 0
-    R.noisy_search(plain, 0, 0, 0, "hash_pos", np.random.RandomState([1, 1]), 0.5, 0.03)     # noise at N = 0: no effect
-    assert np.array_equal(plain.root_children()[2], noisy.root_children()[2])
-    best = int(np.argmax(plain.root_children()[2]))
+    S.noisy_search(plain, 0, 0, 0, "hash_pos", np.random.RandomState([1, 1]), 0.5, 0.03)     # noise at N = 0: no effect
+    assert np.array_equal(plain.root_children()[1], noisy.root_children()[1])
+    best = int(np.argmax(plain.root_children()[1]))
     for t in (plain, noisy):
         t.update(best)
     assert plain.search(1, 0, 200, "hash_pos") == 0
-    R.noisy_search(noisy, 1, 0, 200, "hash_pos", np.random.RandomState([1, 1]), 0.5, 0.03)
-    assert not np.array_equal(plain.root_children()[2], noisy.root_children()[2])
+    S.noisy_search(noisy, 1, 0, 200, "hash_pos", np.random.RandomState([1, 1]), 0.5, 0.03)
+    assert not np.array_equal(plain.root_children()[1], noisy.root_children()[1])
 
 
 def test_games_file_refusals(tmp_path):
@@ -190,7 +187,7 @@ def test_games_file_refusals(tmp_path):
     B = 2
 
     def mk(noise):
-        return SelfPlay(B, lambda x: None, 8, seeds=[3, 4], engine=R.StandIn(B, "hash_pos"), root_noise=noise)
+        return SelfPlay(B, lambda x: None, 8, seeds=[3, 4], engine=S.StandIn(B, "hash_pos"), root_noise=noise)
     on, off = mk((0.25, 0.3)), mk(None)
     on.step()
     off.step()

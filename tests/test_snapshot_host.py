@@ -247,15 +247,12 @@ def test_offsets_must_be_monotone_and_name_the_game():
 
 
 def test_save_games_round_trips_the_host_state_of_every_slot(tmp_path):
-    """SelfPlay.save_games / load_games on the CPU (the engine replaced by the oracle trees, its blob by a marker): boards, sides,
-    live, RNG states, plies and every slot's unfinished record come back, and the records materialise the same tuples."""
-    import os
-    import sys
-    sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-    from test_host import _OracleEngine
+    """SelfPlay.save_games / load_games on the CPU (the engine replaced by the specification trees, its blob by a marker): boards,
+    sides, live, RNG states, plies and every slot's unfinished record come back, and the records materialise the same tuples."""
+    from search_spec import StandIn
     from cchess_zero_b200.selfplay import SelfPlay
 
-    class Eng(_OracleEngine):
+    class Eng(StandIn):
         def snapshot(self):
             return np.arange(40, dtype=np.uint8)
 

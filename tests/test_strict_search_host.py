@@ -9,7 +9,7 @@ import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
-import strict_search_support as S  # noqa: E402
+import search_spec as S  # noqa: E402
 from strict_support import mask_bits, oracle_strict, random_play, setup_boards  # noqa: E402
 from test_snapshot_host import F_CUR, NONE, blob, block, check, game, mv, tree  # noqa: E402
 
@@ -23,7 +23,7 @@ def O():
 def _children(board, side):
     """The spec's children of a position: its root expansion (a search of 0 playouts).  Set-up boards may hold moves without a label
     (error 2) or more than 128 pseudo-legal moves (error 16), as on the device."""
-    t = S.StrictTree(board)
+    t = S.Tree(board, "strict")
     assert t.search(side, 0, 0, "hash_pos") & ~(2 | 16) == 0
     return t.root_children()[0], t
 
@@ -59,7 +59,7 @@ def test_hand_made_mates_in_one(O):
         assert len(S.strict_moves(nb, s ^ 1)) == 0 and S.in_check(nb, s ^ 1) == (not stalemate), name
         assert mate in [O.move_str(x) for x in S.strict_moves(b, s)], name
         for net in S.NETS:
-            t = S.StrictTree(b)
+            t = S.Tree(b, "strict")
             assert t.search(s, 0, 200, net) == 0
             m, N, W, P, Q = t.root_children()
             sig = t.signature()
@@ -73,7 +73,7 @@ def test_hand_made_mates_in_one(O):
                     assert Q[i] == np.float32(1.0) and W[i] == np.float32(N[i]), (name, net, labels[i])
                     r = sig[rec[i]]
                     assert r[5] == -1 and r[4] == np.float32(1.0).view(np.uint32) and r[1] == N[i], (name, net, labels[i])
-                    assert S.game_end(child, s ^ 1, 0) == (3, s), name
+                    assert S.game_end(child, s ^ 1, 0, "strict") == (3, s), name
                     found += 1
             # hash_pos priors are all positive, so every root child is tried; the signed nets may leave a mate unvisited
             assert found or net != "hash_pos", (name, net)
@@ -98,12 +98,12 @@ def test_mated_root_has_no_search(O):
     for name, state, side, mate, _ in S.MATE_IN_ONE:
         b, s = O.from_state(state), 0 if side == "w" else 1
         nb, _ = O.apply_move(b, O.move_from_str(mate))
-        t = S.StrictTree(nb)
+        t = S.Tree(nb, "strict")
         assert t.search(s ^ 1, 0, 100, "hash_pos") == 0
         st = t.stats()
         assert t.root_mated() and st["n_expand"] == 1 and st["n_playout"] == 0 and st["sum_C"] == 0, name
         assert len(t.signature()) == 0 and len(t.root_children()[0]) == 0
-        assert S.game_end(nb, s ^ 1, 0) == (3, s), name
+        assert S.game_end(nb, s ^ 1, 0, "strict") == (3, s), name
 
 
 def test_stalemate_loses():
@@ -112,7 +112,7 @@ def test_stalemate_loses():
     b = O.from_state(state)
     nb, _ = O.apply_move(b, O.move_from_str(mate))
     assert stalemate and not S.in_check(nb, 0)
-    end, winner = S.game_end(nb, 0, 0)
+    end, winner = S.game_end(nb, 0, 0, "strict")
     assert (end, winner) == (3, 1)                                   # red has no move: black, who just moved, wins
 
 
@@ -184,109 +184,17 @@ def test_format_2_refusals_each_with_its_own_message():
 
 
 # ---- the host side of SelfPlay, Match and Trainer under strict rules ------------------------------------------------------------
-class StrictStandIn:
-    """Engine-interface stand-in over the specification trees, with strict rules: a new root without a strictly legal move ends the
-    game with terminal code 3 (the winner is the side that just moved).  Test infrastructure only."""
-    torch_device = "cpu"
-    rules = "strict"
-
-    def __init__(self, n, net):
-        from oracle import oracle as O
-        self.O, self.B, self.net, self.device, self.launches = O, n, net, 0, 0
-        self.boards = np.tile(O.from_state(O.START), (n, 1))
-        self.trees = [S.StrictTree(self.boards[g]) for g in range(n)]
-        self.side = np.zeros(n, np.uint8); self.rr = np.zeros(n, np.int32); self.ply = np.zeros(n, np.int32)
-        self.terminal = np.zeros(n, np.uint8); self.winner = -np.ones(n, np.int8)
-        self.target = np.zeros(n, np.int64); self.pending = np.zeros(n, bool)
-
-    def reset(self, mask=None, boards=None, sides=None, rr=None):
-        for g in range(self.B):
-            if mask is None or mask[g]:
-                self.boards[g] = self.O.from_state(self.O.START) if boards is None else boards[g]
-                self.side[g] = 0 if sides is None else sides[g]
-                self.rr[g] = 0 if rr is None else rr[g]
-                self.trees[g] = S.StrictTree(self.boards[g])
-                self.ply[g] = 0; self.terminal[g] = 0; self.winner[g] = -1
-                self._mate(g)
-
-    def _mate(self, g):
-        if self.terminal[g] == 0 and len(S.strict_moves(self.boards[g], int(self.side[g]))) == 0:
-            self.terminal[g], self.winner[g] = 3, self.side[g] ^ 1
-
-    def begin_search(self, playouts, mask=None):
-        for g in range(self.B):
-            if (mask[g] if mask is not None else not self.terminal[g]):
-                self.target[g] = playouts; self.pending[g] = True
-
-    def wave(self, nn_in, logits, value):
-        for g in np.nonzero(self.pending)[0]:
-            assert self.trees[g].search(int(self.side[g]), int(self.rr[g]), int(self.target[g]), self.net) == 0
-        self.pending[:] = False
-
-    def unfinished(self):
-        return int(self.pending.sum())
-
-    def root_children(self, want_wpq=True):
-        n = np.zeros(self.B, np.int32); m = np.zeros((self.B, 128), np.uint16); v = np.zeros((self.B, 128), np.int32)
-        for g, t in enumerate(self.trees):
-            a, N = t.root_children()[:2]
-            n[g] = len(a); m[g, :len(a)] = a; v[g, :len(a)] = N
-        return dict(n=n, moves=m, visits=v, w=None, p=None, q=None)
-
-    def _advance(self, g, move):
-        self.boards[g], cap = self.O.apply_move(self.boards[g], int(move))
-        self.side[g] ^= 1; self.rr[g] = self.rr[g] + 1 if cap == 0 else 0; self.ply[g] += 1
-        if cap == 1: self.terminal[g], self.winner[g] = 1, 1
-        elif cap == 8: self.terminal[g], self.winner[g] = 1, 0
-        elif self.rr[g] >= 60: self.terminal[g] = 2
-        self._mate(g)
-
-    def play(self, choice, want_status=True):
-        for g, c in enumerate(choice):
-            if c >= 0:
-                move = self.trees[g].root_children()[0][c]
-                self.trees[g].update(int(c))
-                self._advance(g, move)
-        return self.status()
-
-    def play_moves(self, moves, want_status=True):
-        for g, m in enumerate(moves):
-            if m == 0xFFFF:
-                continue
-            kids = list(self.trees[g].root_children()[0])
-            assert self.terminal[g] == 0 and int(m) in [int(x) for x in S.strict_moves(self.boards[g], int(self.side[g]))]
-            if kids:
-                self.trees[g].update(kids.index(m))
-                self._advance(g, m)
-            else:
-                self._advance(g, m)
-                self.trees[g] = S.StrictTree(self.boards[g])
-        return self.status()
-
-    def status(self, boards=True):
-        return dict(terminal=self.terminal.copy(), winner=self.winner.copy(), ply=self.ply.copy(), rr=self.rr.copy(),
-                    side=self.side.copy(), boards=self.boards.copy(), q=np.zeros(self.B, np.float32))
-
-    def counters(self):
-        return dict(error=0)
-
-    def raise_on_error(self):
-        return self.counters()
-
-    def tree_signature(self, g):
-        return self.trees[g].signature()
-
-
 def test_selfplay_host_loop_ends_mated_games_with_the_winners_z():
     from cchess_zero_b200.selfplay import SelfPlay
     B, P, net = 4, 24, "hash_pos"
-    sp = SelfPlay(B, lambda x: None, P, seeds=[500 + g for g in range(B)], auto_reset=False, engine=StrictStandIn(B, net), rules="strict")
+    sp = SelfPlay(B, lambda x: None, P, seeds=[500 + g for g in range(B)], auto_reset=False, engine=S.StandIn(B, net, "strict"),
+                  rules="strict")
     with np.errstate(all="ignore"):
         out = sp.play_games()
     ends = []
     for slot, rec in out:
         with np.errstate(all="ignore"):
-            r = S.selfplay_game(net, P, np.random.RandomState(500 + slot))
+            r = S.selfplay_game(net, P, np.random.RandomState(500 + slot), rules="strict")
         assert rec.states == r["states"] and rec.actions == r["actions"], slot
         assert np.array_equal(rec.z, r["z"]) and np.array_equal(rec.dense_pi(), r["pis"]), slot
         ends.append(r["end"])
@@ -302,7 +210,7 @@ def test_match_host_loop_counts_a_mate_as_a_win(monkeypatch):
 
     class SP(SelfPlay):
         def __init__(self, n, evaluator, playouts, **kw):
-            super().__init__(n, lambda x: None, playouts, engine=StrictStandIn(n, nets[evaluator]), **kw)
+            super().__init__(n, lambda x: None, playouts, engine=S.StandIn(n, nets[evaluator], "strict"), **kw)
 
         def capture_graph(self, warmup=3):
             pass
@@ -315,7 +223,7 @@ def test_match_host_loop_counts_a_mate_as_a_win(monkeypatch):
     for g in range(n):
         red, black = ("hash_signed", "mod17") if g < n // 2 else ("mod17", "hash_signed")
         with np.errstate(all="ignore"):
-            o = S.match_game(red, black, P, np.random.RandomState(g), plies0, T0, 1e-3, max_plies=400)
+            o = S.match_game(red, black, P, np.random.RandomState(g), plies0, T0, 1e-3, max_plies=400, rules="strict")
         rec = r.games[g]
         assert rec["moves"] == o["moves"] and rec["winner"] == "wbt"[o["winner"]] and rec["plies"] == o["plies"], g
         ends.append(o["end"])
@@ -332,7 +240,7 @@ def test_strict_match_ends_a_mated_opening_before_its_first_ply(monkeypatch):
 
     class SP(SelfPlay):
         def __init__(self, n, evaluator, playouts, **kw):
-            super().__init__(n, lambda x: None, playouts, engine=StrictStandIn(n, evaluator), **kw)
+            super().__init__(n, lambda x: None, playouts, engine=S.StandIn(n, evaluator, "strict"), **kw)
 
         def capture_graph(self, warmup=3):
             pass
@@ -375,7 +283,7 @@ def test_rules_argument_is_validated():
     with pytest.raises(ValueError, match="rules must be"):
         random_openings(2, 2, rules="xiangqi")
     with pytest.raises(ValueError, match="plays by the 'strict' rules"):
-        SelfPlay(2, lambda x: None, 8, engine=StrictStandIn(2, "hash_pos"))
+        SelfPlay(2, lambda x: None, 8, engine=S.StandIn(2, "hash_pos", "strict"))
 
 
 def test_trainer_refuses_a_saved_run_of_other_rules(tmp_path):
