@@ -22,9 +22,9 @@ import numpy as np
 import torch
 
 from . import rules as _rules                        # (random_openings and Match take a `rules` argument)
-from ._lib import MT_WORDS, NLABEL, TERM_MATED, EngineError
+from ._lib import NLABEL, TERM_MATED, EngineError
 from .engine import check_rules
-from .selfplay import SelfPlay, network_selfplay, sample_moves
+from .selfplay import SelfPlay, mt_streams, network_selfplay, sample_moves
 
 NO_MOVE = 0xFFFF
 
@@ -168,11 +168,9 @@ class Match:
                         _Player(best, h, playouts, search_threads, arena_words, 1, 0, self.rules),
                         _Player(candidate, h, playouts, search_threads, arena_words, 1, h, self.rules),
                         _Player(best, h, playouts, search_threads, arena_words, 0, h, self.rules)]
-        seeds = range(self.n) if seeds is None else seeds
-        self._mt = np.zeros((self.n, MT_WORDS), dtype=np.uint32)
-        for g, sd in enumerate(seeds):
-            st = np.random.RandomState(int(sd)).get_state()
-            self._mt[g, :624], self._mt[g, 624] = st[1], st[2]
+        self._mt = mt_streams(range(self.n) if seeds is None else seeds)
+        if len(self._mt) != self.n:
+            raise ValueError("Match: %d seeds for %d games" % (len(self._mt), self.n))
         if openings is None:
             ob = _rules.state_to_board(_rules.START_STATE)[None]
             os_, orr = np.zeros(1, np.uint8), np.zeros(1, np.int32)

@@ -18,20 +18,9 @@ O_SIDE, O_N, O_IDX, O_PROB, O_Z = 90, 91, 96, 96 + 2 * MAXC, 96 + 2 * MAXC + 8 *
 REC_BYTES = O_Z + 8
 
 
-def _flip_boards(b):
-    """try_flip (main.py:560-574) for a stack of boards [L,90]: rows reversed, colours swapped."""
-    f = b.reshape(-1, 10, 9)[:, ::-1].copy()
-    red, blk = (f >= 1) & (f <= 7), f >= 8
-    f[red] += 7
-    f[blk] -= 7
-    return f.reshape(-1, 90)
-
-
 def pack_records(records, cap=None):
     """records: iterable of GameRecord (selfplay.py).  Returns (uint8 [n, REC_BYTES], n, leftover records): with cap=None
     every tuple is packed; with a cap whole trailing games that do not fit are handed back, never dropped."""
-    from . import rules
-    from .selfplay import _label_table
     rows, n, left = [], 0, []
     records = list(records)
     for k, r in enumerate(records):
@@ -41,41 +30,14 @@ def pack_records(records, cap=None):
             break
         if L == 0:
             continue
+        p = r.positions()
         buf = np.zeros((L, REC_BYTES), dtype=np.uint8)
-        r._raw() if hasattr(r, "_raw") and r._boards is None else None
-        if r._boards and r._boards[0] is not None:               # raw per-ply data of a game played here
-            boards = np.stack(r._boards).astype(np.uint8)
-            sides = np.asarray(r.players, dtype=np.uint8)
-            canon = np.where((sides == 1)[:, None], _flip_boards(boards), boards)
-            tab = _label_table()
-            idx_rows = []
-            for mv, side in zip(r._moves, sides):
-                src, dst = (mv & 127).astype(np.int64), (mv >> 7).astype(np.int64)
-                if side == 1:                                       # flipped_uci_labels for black (main.py:1507-1512)
-                    src = (9 - src // 9) * 9 + src % 9
-                    dst = (9 - dst // 9) * 9 + dst % 9
-                li = tab[src, dst]
-                if (li < 0).any():
-                    raise KeyError("move outside the label table")
-                idx_rows.append(li)
-        else:                                                        # a record built from materialised tuples
-            canon = np.stack([rules.state_to_board(s) for s in r.states]).astype(np.uint8)
-            sides = np.zeros(L, dtype=np.uint8)
-            idx_rows = r.pi_idx
-        buf[:, :90] = canon
-        buf[:, O_SIDE] = sides
-        cnt = np.fromiter((len(ix) for ix in idx_rows), dtype=np.int64, count=L)
-        if (cnt > MAXC).any():
-            raise ValueError("more than %d moves in one position" % MAXC)
-        buf[:, O_N] = cnt
-        idx = np.zeros((L, MAXC), dtype=np.int16)
-        prob = np.zeros((L, MAXC), dtype=np.float64)
-        for i, (ix, pv) in enumerate(zip(idx_rows, r.pi_val)):
-            idx[i, :len(ix)] = ix
-            prob[i, :len(ix)] = pv
-        buf[:, O_IDX:O_PROB] = idx.view(np.uint8)
-        buf[:, O_PROB:O_Z] = prob.view(np.uint8)
-        buf[:, O_Z:] = np.asarray(r.z, dtype=np.float64).reshape(L, 1).view(np.uint8)
+        buf[:, :90] = p.boards
+        buf[:, O_SIDE] = p.sides
+        buf[:, O_N] = p.n
+        buf[:, O_IDX:O_PROB] = p.idx.view(np.uint8)
+        buf[:, O_PROB:O_Z] = p.prob.view(np.uint8)
+        buf[:, O_Z:] = p.z.reshape(L, 1).view(np.uint8)
         rows.append(buf)
         n += L
     out = np.concatenate(rows) if rows else np.zeros((0, REC_BYTES), dtype=np.uint8)

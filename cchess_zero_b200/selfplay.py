@@ -7,35 +7,70 @@ np.random.choice(p = 0.75*pi + 0.25*Dirichlet(0.3)) on a legacy MT19937 RandomSt
 RandomState per game slot stands in for the reference's global np.random (SURVEY H3).  The device
 produces the integer visit counts; everything before them (select / expand / backup / encode /
 move generation / re-rooting) runs in csrc/cz_engine.cu."""
+import ctypes as C
 import os
 import pickle
 import random
 import time
+import types
 from collections import defaultdict, deque
 
 import numpy as np
 import torch
 
 from . import rules as _rules                        # (SelfPlay takes a `rules` argument)
-from ._lib import MAXCHILD, MT_WORDS, NLABEL, NSQ, TERM_MATED, EngineError
+from ._lib import MAXCHILD, MT_WORDS, NLABEL, NSQ, TERM_MATED, EngineError, lib
 from .engine import Engine, capture_cuda_graph, check_rules, run_waves
 
 
+def _vp(a):
+    return a.ctypes.data_as(C.c_void_p)
+
+
 def _flip_board(b):
-    """try_flip (main.py:560-574): reverse the rows, swap the colours; files are not mirrored."""
-    f = b.reshape(10, 9)[::-1].copy()
+    """try_flip (main.py:560-574) for one board [90] or a stack [L,90]: reverse the rows, swap the colours; files are not mirrored."""
+    f = b.reshape(-1, 10, 9)[:, ::-1].copy()
     red, blk = (f >= 1) & (f <= 7), f >= 8
     f[red] += 7
     f[blk] -= 7
-    return f.reshape(90)
+    return f.reshape(b.shape)
 
 
-def _flip_move_label_index(mv):
-    """label index of the rank-mirrored move (flipped_uci_labels, main.py:23-27 / 1507-1512)."""
-    s, d = int(mv) & 127, (int(mv) >> 7) & 127
-    s = (9 - s // 9) * 9 + s % 9
-    d = (9 - d // 9) * 9 + d % 9
-    return _rules.label2i[_rules.move_to_label(s | (d << 7))]
+def _flip_move_label_index(moves, flip=True):
+    """Label index of every u16 move code in `moves`; where `flip` (broadcast against moves; by default every move) is set, of the
+    rank-mirrored move (y -> 9 - y: flipped_uci_labels for black, main.py:23-27 / 1507-1512).  KeyError, as label2i[...] in the
+    reference, when a move is not a label."""
+    mv = np.asarray(moves).astype(np.int64)
+    src, dst = mv & 127, (mv >> 7) & 127
+    flip = np.asarray(flip, dtype=bool)
+    src = np.where(flip, (9 - src // 9) * 9 + src % 9, src)
+    dst = np.where(flip, (9 - dst // 9) * 9 + dst % 9, dst)
+    li = _label_table()[src, dst]
+    if (li < 0).any():
+        raise KeyError("move outside the label table")
+    return li
+
+
+def visit_exp(n, visits, temperature):
+    """The rows of pi = softmax(1/T * log(visits)) (main.py:1341, 1111-1116) before their sums: exp(lv - max(lv)) with
+    lv = 1/T * log(visits) in float64, -inf (exp 0) past each row's n.  n [L], visits [L,128]; temperature: a scalar or one value per
+    row.  log / exp / max are element-wise or exact, so they are taken over the whole batch at once; the order-sensitive row sums are
+    cz_host_choose_moves', operation for operation what numpy does for `probs /= np.sum(probs)`."""
+    inv_t = (1.0 / temperature) if np.ndim(temperature) == 0 else (1.0 / np.asarray(temperature, dtype=np.float64))[:, None]
+    with np.errstate(divide="ignore", invalid="ignore"):
+        lv = inv_t * np.log(visits.astype(np.int64))
+        lv[np.arange(MAXCHILD)[None, :] >= n[:, None]] = -np.inf
+        return np.ascontiguousarray(np.exp(lv - np.max(lv, axis=1, keepdims=True)))
+
+
+def mt_streams(seeds, key=None):
+    """One legacy MT19937 stream per seed, RandomState(seed) (or RandomState([seed, key])), as raw numpy RandomState states
+    uint32 [len(seeds), 626]: csrc/cz_host.cu draws from them exactly as RandomState.dirichlet / .choice would."""
+    mt = np.zeros((len(seeds), MT_WORDS), dtype=np.uint32)
+    for g, sd in enumerate(seeds):
+        st = np.random.RandomState(int(sd) if key is None else [int(sd), key]).get_state()
+        mt[g, :624], mt[g, 624] = st[1], st[2]
+    return mt
 
 
 _LABEL_OF = None
@@ -45,7 +80,6 @@ def _label_table():
     """(src_sq, dst_sq) -> label index as a numpy table (cz_label_index); -1 where the pair is not a label."""
     global _LABEL_OF
     if _LABEL_OF is None:
-        from ._lib import lib
         L = lib()
         _LABEL_OF = np.array([[L.cz_label_index(s, d) for d in range(90)] for s in range(90)], dtype=np.int64)
     return _LABEL_OF
@@ -74,25 +108,15 @@ def sample_moves(n_children, visits, live, temperature, mt_states, exploration, 
     scalar or one value per game; mt_states [B,626]: one legacy MT19937 state per game, advanced in place.  Returns choice [B] int32."""
     B = len(n_children)
     choice = np.full(B, -1, dtype=np.int32)
-    inv_t = (1.0 / temperature) if np.ndim(temperature) == 0 else (1.0 / np.asarray(temperature, dtype=np.float64))[:, None]
-    with np.errstate(divide="ignore", invalid="ignore"):
-        # softmax(1/T * log(visits)) of main.py:1341, 1111-1116.  log / exp / max are element-wise or exact, so they are
-        # taken over the whole [B,128] batch at once (padding: visits 0 -> -inf -> exp 0); the order-sensitive row sum, the
-        # Dirichlet / choice draws and the cumulative sums happen per game in csrc/cz_host.cu, operation for operation what
-        # numpy does for `probs /= np.sum(probs)`, RandomState.dirichlet and RandomState.choice (main.py:1345-1348).
-        lv = inv_t * np.log(visits.astype(np.int64))
-        valid = np.arange(MAXCHILD)[None, :] < n_children[:, None]
-        lv[~valid] = -np.inf
-        ex = np.ascontiguousarray(np.exp(lv - np.max(lv, axis=1, keepdims=True)))
+    # pi's rows (visit_exp); the row sums, the Dirichlet / choice draws and the cumulative sums happen per game in csrc/cz_host.cu,
+    # operation for operation what numpy does for RandomState.dirichlet and RandomState.choice (main.py:1345-1348)
+    ex = visit_exp(n_children, visits, temperature)
     probs = np.empty((B, MAXCHILD), dtype=np.float64)
     fallback = np.zeros(B, dtype=np.uint8)
     live8 = np.ascontiguousarray(live, dtype=np.uint8)
     nn = np.ascontiguousarray(n_children, dtype=np.int32)
-    from ._lib import lib
-    import ctypes as C
-    vp = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
-    rcode = lib().cz_host_choose_moves(B, vp(live8), vp(nn), vp(ex), 1 if exploration else 0, vp(mt_states), vp(choice), vp(probs),
-                                       vp(fallback), n_threads)
+    rcode = lib().cz_host_choose_moves(B, _vp(live8), _vp(nn), _vp(ex), 1 if exploration else 0, _vp(mt_states), _vp(choice), _vp(probs),
+                                       _vp(fallback), n_threads)
     if rcode:
         raise EngineError("cz_host_choose_moves failed (%d)" % rcode)
     for g in np.nonzero(fallback)[0]:
@@ -107,106 +131,110 @@ def sample_moves(n_children, visits, live, temperature, mt_states, exploration, 
     return choice
 
 
+# one log entry per ply (SelfPlay.step), for the whole batch: (field, shape per game, dtype)
+_LOG = (("boards", (NSQ,), np.uint8), ("n", (), np.int32), ("moves", (MAXCHILD,), np.uint16), ("visits", (MAXCHILD,), np.int32),
+        ("choice", (), np.int32))
+
+
 class GameRecord:
     """(s, pi, z) tuples of one finished game in the reference's format (selfplay, main.py:1493-1554).
 
-    During play nothing per game is recorded: SelfPlay keeps ONE log entry per ply for the whole batch (boards, sides, root moves
-    and visit counts, chosen indices); a record only remembers its slot and ply span.  Boards, move lists, pi (recomputed from the
-    integer visit counts with the very numpy operations get_action uses, so bit-identical) and the canonical state strings /
-    label indices are materialised on first access."""
+    During play nothing per game is recorded: SelfPlay keeps ONE log entry per ply for the whole batch (boards, root moves and
+    visit counts, chosen indices); a record only remembers its slot, ply span, players and temperature.  positions() turns them into
+    the game's training positions on first use; pi is recomputed from the integer visit counts with the very numpy operations
+    get_action uses, so bit-identical."""
 
     def __init__(self, slot=None, logs=None, temperature=1):
         self._slot, self._logs, self._T = slot, logs if logs is not None else [], temperature
         self.players = []
         self.z = None
         self.winner = None
-        self._boards = self._moves = self._chosen = self.visits = self.pi_val = None
-        self._states = self._pi_idx = self._actions = None
+        self._log = self._pos = self._states = None
 
     def __len__(self):
         return len(self.players)
 
-    def _raw(self):
-        if self._boards is not None:
-            return
-        g = self._slot
-        logs = self._logs
-        L = len(logs)
-        self._boards = [lg["boards"][g] for lg in logs]
-        nn = np.fromiter((lg["n"][g] for lg in logs), dtype=np.int32, count=L)
-        self._chosen = [int(lg["choice"][g]) for lg in logs]
-        V = np.stack([lg["visits"][g] for lg in logs]) if L else np.zeros((0, MAXCHILD), np.int32)
-        M = np.stack([lg["moves"][g] for lg in logs]) if L else np.zeros((0, MAXCHILD), np.uint16)
-        self._moves = [M[i, :nn[i]] for i in range(L)]
-        self.visits = [V[i, :nn[i]] for i in range(L)]
-        # pi = softmax(1/T * log(visits)) (main.py:1341, 1111-1116): element-wise log / exp for the whole game at once, the
-        # order-sensitive row sums in csrc/cz_host.cu exactly as np.sum does them (the same call get_action's batch path uses)
-        with np.errstate(divide="ignore", invalid="ignore"):
-            lv = (1.0 / self._T) * np.log(V.astype(np.int64))
-            lv[np.arange(MAXCHILD)[None, :] >= nn[:, None]] = -np.inf
-            ex = np.ascontiguousarray(np.exp(lv - np.max(lv, axis=1, keepdims=True))) if L else np.zeros((0, MAXCHILD))
-        probs = np.empty((L, MAXCHILD), dtype=np.float64)
-        if L:
-            import ctypes as C
-            from ._lib import lib
-            vp = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
+    def _log_arrays(self):
+        """This slot's log span as arrays: boards [L,90], n [L], moves [L,128], visits [L,128], choice [L]."""
+        if self._log is None:
+            g, L = self._slot, len(self._logs)
+            self._log = {k: np.array([lg[k][g] for lg in self._logs], dtype=dt).reshape((L,) + shp) for k, shp, dt in _LOG}
+            self._logs = None
+        return self._log
+
+    def positions(self):
+        """The game's training positions, in the fields of distributed.TupleBatch plus sides: boards u8 [L,90] (side to move
+        canonical, main.py:1504-1505), sides u8 [L], n [L], idx i16 [L,128] (label indices, black's ranks flipped: main.py:1507-1512),
+        prob f64 [L,128] (pi) and z f64 [L]; idx and prob are 0 past n."""
+        if self._pos is None:
+            r = self._log_arrays()
+            n, L = r["n"], len(r["n"])
+            sides = np.asarray(self.players, dtype=np.uint8)
+            valid = np.arange(MAXCHILD)[None, :] < n[:, None]
+            idx = np.zeros((L, MAXCHILD), dtype=np.int16)
+            idx[valid] = _flip_move_label_index(r["moves"][valid], np.repeat(sides == 1, n))
+            # pi = softmax(1/T * log(visits)) at this slot's temperature; the row sums are get_action's batch path (sample_moves)
+            T = self._T if np.ndim(self._T) == 0 else np.asarray(self._T, dtype=np.float64)[self._slot]
+            ex = visit_exp(n, r["visits"], T)
+            prob = np.zeros((L, MAXCHILD), dtype=np.float64)
             mt = np.zeros((L, MT_WORDS), dtype=np.uint32); mt[:, 624] = 624          # scratch generators: the draws are discarded
             ch, fb = np.zeros(L, np.int32), np.zeros(L, np.uint8)
-            lib().cz_host_choose_moves(L, None, vp(nn), vp(ex), 0, vp(mt), vp(ch), vp(probs), vp(fb), 1)
+            lib().cz_host_choose_moves(L, None, _vp(n), _vp(ex), 0, _vp(mt), _vp(ch), _vp(prob), _vp(fb), 1)
             for i in np.nonzero(fb)[0]:                                               # (NaN rows: plain numpy, as get_action would)
-                pr = ex[i, :nn[i]].copy(); pr /= np.sum(pr); probs[i, :nn[i]] = pr
-        self.pi_val = [probs[i, :nn[i]] for i in range(L)]
-        self._logs = None
-
-    def _materialise(self):
-        self._raw()
-        if self._states is not None and len(self._states) == len(self.players):
-            return
-        tab = _label_table()
-        st, ix = [], []
-        for b, side, mv in zip(self._boards, self.players, self._moves):
-            st.append(_rules.board_to_state(_flip_board(b) if side == 1 else b))             # main.py:1504-1505
-            src, dst = (mv & 127).astype(np.int64), (mv >> 7).astype(np.int64)
-            if side == 1:   # flipped_uci_labels for black (main.py:1507-1512): rank y -> 9-y
-                src = (9 - src // 9) * 9 + src % 9
-                dst = (9 - dst // 9) * 9 + dst % 9
-            li = tab[src, dst]
-            if (li < 0).any():
-                raise KeyError("move outside the label table")                                # label2i[...] KeyError in the reference
-            ix.append(li)
-        self._states, self._pi_idx = st, ix
-        self._actions = [_rules.move_to_label(mv[c]) for mv, c in zip(self._moves, self._chosen)]
+                pr = ex[i, :n[i]].copy(); pr /= np.sum(pr); prob[i, :n[i]] = pr
+            boards = np.where((sides == 1)[:, None], _flip_board(r["boards"]), r["boards"])
+            self._pos = types.SimpleNamespace(boards=boards, sides=sides, n=n, idx=idx, prob=prob, z=np.asarray(self.z, dtype=np.float64))
+        return self._pos
 
     @classmethod
     def from_tuples(cls, states, pi_idx, pi_val, z):
-        """A record built from already materialised tuples (tests, gathered data)."""
+        """A record built from already materialised tuples (tests, gathered data); its sides are 0."""
         r = cls()
-        r._states, r._pi_idx, r.pi_val, r.z = list(states), list(pi_idx), list(pi_val), z
-        r.players = [0] * len(r._states)
-        r._boards = [None] * len(r._states)
-        r._moves = r._chosen = r.visits = []
+        r._states, r.z = list(states), z
+        L = len(r._states)
+        r.players = [0] * L
+        n = np.fromiter((len(ix) for ix in pi_idx), dtype=np.int32, count=L)
+        if (n > MAXCHILD).any():
+            raise ValueError("more than %d moves in one position" % MAXCHILD)
+        idx, prob = np.zeros((L, MAXCHILD), dtype=np.int16), np.zeros((L, MAXCHILD), dtype=np.float64)
+        for i, (ix, pv) in enumerate(zip(pi_idx, pi_val)):
+            idx[i, :n[i]], prob[i, :n[i]] = ix, pv
+        boards = np.array([_rules.state_to_board(s) for s in r._states], dtype=np.uint8).reshape(L, NSQ)
+        r._pos = types.SimpleNamespace(boards=boards, sides=np.zeros(L, dtype=np.uint8), n=n, idx=idx, prob=prob,
+                                       z=np.asarray(z, dtype=np.float64))
         return r
 
     @property
     def states(self):
-        self._materialise()
+        if self._states is None:
+            self._states = [_rules.board_to_state(b) for b in self.positions().boards]
         return self._states
 
     @property
     def pi_idx(self):
-        self._materialise()
-        return self._pi_idx
+        p = self.positions()
+        return [p.idx[i, :k] for i, k in enumerate(p.n)]
+
+    @property
+    def pi_val(self):
+        p = self.positions()
+        return [p.prob[i, :k] for i, k in enumerate(p.n)]
+
+    @property
+    def visits(self):
+        r = self._log_arrays()
+        return [v[:k] for v, k in zip(r["visits"], r["n"])]
 
     @property
     def actions(self):
-        self._materialise()
-        return self._actions
+        r = self._log_arrays()
+        return [_rules.move_to_label(mv[c]) for mv, c in zip(r["moves"], r["choice"])]
 
     def dense_pi(self):
-        self._raw()
+        p = self.positions()
+        valid = np.arange(MAXCHILD)[None, :] < p.n[:, None]
         out = np.zeros((len(self), NLABEL))
-        for i, (ix, v) in enumerate(zip(self.pi_idx, self.pi_val)):
-            out[i, ix] = v
+        out[np.nonzero(valid)[0], p.idx[valid]] = p.prob[valid]
         return out
 
     def tuples(self):
@@ -271,37 +299,42 @@ class SelfPlay:
         self.plan = plan
         self.forward = forward
         self.playouts = np.broadcast_to(np.asarray(playouts, dtype=np.int64), (n_games,)).copy()
-        seeds = range(n_games) if seeds is None else seeds
-        # one legacy MT19937 stream per game slot (stands in for the reference's global np.random, SURVEY H3), held as raw numpy
-        # RandomState states: csrc/cz_host.cu draws from them exactly as RandomState.dirichlet / .choice would
-        self._mt = np.zeros((n_games, MT_WORDS), dtype=np.uint32)
-        for g, sd in enumerate(seeds):
-            st = np.random.RandomState(int(sd)).get_state()
-            self._mt[g, :624], self._mt[g, 624] = st[1], st[2]
-        # root noise: a second stream per slot, RandomState([seed, 1]), so that the move choice draws stay those of a run without noise
-        self._noise_mt = self._eta = None                  # (and the host buffer of one search's draws, [B, 128])
-        if self.root_noise is not None:
-            self._noise_mt = np.zeros((n_games, MT_WORDS), dtype=np.uint32)
-            for g, sd in enumerate(seeds):
-                st = np.random.RandomState([int(sd), 1]).get_state()
-                self._noise_mt[g, :624], self._noise_mt[g, 624] = st[1], st[2]
-            self._eta = np.zeros((n_games, MAXCHILD), dtype=np.float64)
-        self._span = [[] for _ in range(n_games)]        # the log entries of each slot's current game
         self.exploration = exploration
         self.temperature = temperature
         self.auto_reset = auto_reset
         self.keep_records = keep_records
-        self.records = [GameRecord(g, None, temperature) for g in range(n_games)]
         self._start_board = _rules.state_to_board(_rules.START_STATE)
-        self.boards = np.tile(self._start_board, (n_games, 1))
-        self.sides = np.zeros(n_games, dtype=np.uint8)
-        self.live = np.ones(n_games, dtype=bool)
-        self.finished = []
+        # one legacy MT19937 stream per game slot (stands in for the reference's global np.random, SURVEY H3); with root noise a
+        # second one, RandomState([seed, 1]), so that the move choice draws stay those of a run without noise
+        seeds = range(n_games) if seeds is None else seeds
+        self._eta = None if self.root_noise is None else np.zeros((n_games, MAXCHILD), dtype=np.float64)   # one search's draws
+        self._start_games(mt_streams(seeds), None if self.root_noise is None else mt_streams(seeds, 1))
         self.plies = 0
         self.waves = 0
         self.graph = None
         self._threads = max(1, min(16, (len(os.sched_getaffinity(0)) if hasattr(os, "sched_getaffinity") else 4)))
         _rules._init_tables()
+
+    def _start_games(self, mt, noise_mt):
+        """Host state of a fresh game in every slot: start position, red to move, live, empty records, move streams mt and, with root
+        noise, noise streams noise_mt (uint32 [B, 626] each, see mt_streams)."""
+        B = self.B
+        if (noise_mt is None) != (self.root_noise is None):
+            raise ValueError("noise streams are given if and only if root noise is on")
+        self._mt = np.array(mt, dtype=np.uint32).reshape(B, MT_WORDS)
+        self._noise_mt = None if noise_mt is None else np.array(noise_mt, dtype=np.uint32).reshape(B, MT_WORDS)
+        self._span = [[] for _ in range(B)]             # the log entries of each slot's current game
+        self.records = [GameRecord(g, None, self.temperature) for g in range(B)]
+        self.boards = np.tile(self._start_board, (B, 1))
+        self.sides = np.zeros(B, dtype=np.uint8)
+        self.live = np.ones(B, dtype=bool)
+        self.finished = []
+
+    def restart_games(self, mt, noise_mt=None):
+        """Every slot starts a fresh game from the start position (the engine is reset), drawing its moves from the stream mt[slot]
+        and, with root noise, its noise from noise_mt[slot]."""
+        self.engine.reset()
+        self._start_games(mt, noise_mt)
 
     # -- evaluation step ---------------------------------------------------------------------
     def _eval(self, nn_in):
@@ -394,8 +427,6 @@ class SelfPlay:
         for every searched, live game with n >= 1 root children, in slot order: eta = RandomState([seed, 1]).dirichlet(alpha * ones(n))
         (cz_host_dirichlet) and P' = f32((1 - eps) f64(P) + eps eta) on the device (k_root_noise).  The noised root block is dropped
         by the next play (only the chosen subtree is kept), so games at rest never hold noised priors."""
-        import ctypes as C
-        from ._lib import lib
         e = self.engine
         e.begin_search(0, m.astype(np.uint8))
         self.waves += self._run_waves(0, graph=False)
@@ -404,8 +435,7 @@ class SelfPlay:
         if not sel.any():
             return
         eps, alpha = self.root_noise
-        vp = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
-        rc = lib().cz_host_dirichlet(self.B, vp(sel), vp(n), C.byref(C.c_double(alpha)), vp(self._noise_mt), vp(self._eta), self._threads)
+        rc = lib().cz_host_dirichlet(self.B, _vp(sel), _vp(n), C.byref(C.c_double(alpha)), _vp(self._noise_mt), _vp(self._eta), self._threads)
         if rc:
             raise EngineError("cz_host_dirichlet failed (%d)" % rc)
         e.root_noise(sel, self._eta, eps)
@@ -472,9 +502,6 @@ class SelfPlay:
         return out
 
     # -- games in flight: save and restore between plies ------------------------------------------------
-    _LOG = (("boards", (NSQ,), np.uint8), ("n", (), np.int32), ("moves", (MAXCHILD,), np.uint16), ("visits", (MAXCHILD,), np.int32),
-            ("choice", (), np.int32))
-
     def save_games(self, path):
         """Every game in flight into one np.savez file (written to a temporary file, then renamed): the engine's trees and game state
         (Engine.snapshot) and the host state -- boards, sides, live, the per-slot MT19937 states (and, with root noise, the noise
@@ -485,7 +512,7 @@ class SelfPlay:
         from .train import _savez
         blob = self.engine.snapshot()
         rows = [(lg, g) for g in range(self.B) for lg in self._span[g]]
-        log = {"log_" + k: np.asarray([lg[k][g] for lg, g in rows], dtype=dt).reshape((len(rows),) + shp) for k, shp, dt in self._LOG}
+        log = {"log_" + k: np.asarray([lg[k][g] for lg, g in rows], dtype=dt).reshape((len(rows),) + shp) for k, shp, dt in _LOG}
         players = [self.records[g].players for g in range(self.B)]
         if self.root_noise is not None:
             log["noise_mt"] = self._noise_mt
@@ -505,7 +532,7 @@ class SelfPlay:
                     mt=((B, MT_WORDS), np.uint32), plies=((), np.int64), span_len=((B,), np.int64), players_len=((B,), np.int64),
                     players=(None, np.uint8), temperature=(None, np.float64))
         rows = int(a["span_len"].sum()) if "span_len" in a else -1
-        for k, shp, dt in self._LOG:
+        for k, shp, dt in _LOG:
             want["log_" + k] = ((rows,) + shp, dt)
         if ("noise_mt" in a) != (self.root_noise is not None):        # the noise streams are part of an exact resume
             raise ValueError("games file: saved %s root noise, this SelfPlay runs %s" % (("with", "without") if "noise_mt" in a
@@ -527,11 +554,11 @@ class SelfPlay:
         self.engine.restore(a["engine"])                     # validated as a whole before anything on the device is written
         spans = a["span_len"]
         L = int(spans.max()) if B else 0
-        entries = [{k: np.zeros((B,) + shp, dtype=dt) for k, shp, dt in self._LOG} for _ in range(L)]
+        entries = [{k: np.zeros((B,) + shp, dtype=dt) for k, shp, dt in _LOG} for _ in range(L)]
         r = 0
         for g in range(B):                                   # a slot's span is the last span_len[g] plies: align them at the end
             for j in range(L - int(spans[g]), L):
-                for k, _, _ in self._LOG:
+                for k, _, _ in _LOG:
                     entries[j][k][g] = a["log_" + k][r]
                 r += 1
         t = a["temperature"]

@@ -476,23 +476,7 @@ class Trainer:
         if os.path.isfile(games):
             self.sp.load_games(games)
         else:
-            self._restart_games(mt, noise_mt)
-
-    def _restart_games(self, mt, noise_mt=None):
-        """Every slot starts a fresh game from the start position, drawing its moves from the stream mt[slot] (and its root noise
-        from noise_mt[slot])."""
-        from .selfplay import GameRecord
-        sp = self.sp
-        sp.engine.reset()
-        sp._mt[:] = mt
-        if noise_mt is not None:
-            sp._noise_mt[:] = noise_mt
-        sp._span = [[] for _ in range(sp.B)]
-        sp.records = [GameRecord(g, None, sp.temperature) for g in range(sp.B)]
-        sp.boards = np.tile(sp._start_board, (sp.B, 1))
-        sp.sides = np.zeros(sp.B, dtype=np.uint8)
-        sp.live = np.ones(sp.B, dtype=bool)
-        sp.finished = []
+            self.sp.restart_games(mt, noise_mt)
 
 
 def main(argv=None):

@@ -383,6 +383,55 @@ def test_selfplay_auto_reset_path_on_cpu_stand_in_engine():
         assert rec.states == r["states"] and np.array_equal(rec.z, r["z"]) and np.array_equal(rec.dense_pi(), r["pis"])
 
 
+@pytest.mark.parametrize("rules", ["reference", "strict"])
+def test_packed_played_games_equal_the_specification(rules):
+    """pack_records of whole played games (stand-in engine, root noise on), as the Trainer packs them: the packed batch holds the
+    specification's (state, pi, z) and player of every position of the same games, and validate_tuples accepts it."""
+    import search_spec as S
+    from cchess_zero_b200.distributed import O_SIDE, TupleBatch, pack_records
+    from cchess_zero_b200.selfplay import SelfPlay
+    from cchess_zero_b200.train import validate_tuples
+    B, P, net, eps, alpha = 3, 16, "hash_signed", 0.25, 0.3
+    seeds = [600 + 17 * g for g in range(B)]
+    sp = SelfPlay(B, lambda x: None, P, seeds=seeds, auto_reset=False, engine=StandIn(B, net, rules), rules=rules, root_noise=(eps, alpha))
+    with np.errstate(all="ignore"):
+        out = sp.play_games()
+    assert [g for g, _ in out] == list(range(B))
+    buf, n, left = pack_records([rec for _, rec in out])
+    tb = TupleBatch(buf)
+    validate_tuples(tb)
+    want, players = [], []
+    for slot, _ in out:
+        with np.errstate(all="ignore"):
+            r = S.selfplay_game(net, P, np.random.RandomState(seeds[slot]), rules=rules,
+                                root_noise=(eps, alpha, np.random.RandomState([seeds[slot], 1])))
+        want += list(zip(r["states"], r["pis"], r["z"]))
+        players += r["players"]
+    got = tb.tuples()
+    assert n == len(got) == len(want) and not left and (np.asarray(players) == 1).any()
+    assert np.array_equal(buf[:, O_SIDE], players)
+    for (s, pi, z), (s0, p0, z0) in zip(got, want):
+        assert s == s0 and np.array_equal(pi, p0) and z == z0
+
+
+def test_records_use_their_own_slot_temperature():
+    """SelfPlay with one temperature per game: every record's pi is numpy's softmax(1/T[slot] * log(visits)) at its own slot's T."""
+    from cchess_zero_b200.selfplay import SelfPlay
+    B, T = 3, np.array([1.0, 0.5, 2.0])
+    sp = SelfPlay(B, lambda x: None, 16, seeds=[5, 6, 7], auto_reset=False, engine=StandIn(B, "hash_pos"), temperature=T)
+    with np.errstate(all="ignore"):
+        out = sp.play_games()
+    assert [g for g, _ in out] == list(range(B))
+    for slot, rec in out:
+        assert len(rec.states) == len(rec.visits) == len(rec.pi_val) == len(rec) > 0
+        for v, p in zip(rec.visits, rec.pi_val):
+            with np.errstate(divide="ignore"):
+                x = 1.0 / T[slot] * np.log(v)
+            want = np.exp(x - np.max(x))
+            want /= np.sum(want)
+            assert np.array_equal(p, want), slot
+
+
 def test_torch_stand_in_nets_match_oracle_on_cpu():
     """cchess_zero_b200/fakenet.py (torch integer ops, used on the device in the GPU tests) evaluated on CPU tensors against
     the oracle's C restatement and the numpy original."""
