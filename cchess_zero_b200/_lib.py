@@ -10,6 +10,7 @@ NSQ, NLABEL, MAXCHILD, ENC_LEN, STATUS_BYTES, MT_WORDS = 90, 2086, 128, 1260, 11
 F32, BF16, F16, BOARD = 0, 1, 2, 3
 ERR_NAMES = {1: "NOMOVES", 2: "NOLABEL", 4: "DEPTH", 8: "ARENA", 16: "CHILDREN", 32: "ILLEGAL"}
 RULES = {"reference": 0, "strict": 1}     # CZ_RULES_REFERENCE / CZ_RULES_STRICT
+PRIORS = {"reference": 0, "softmax": 1}   # CZ_PRIORS_REFERENCE / CZ_PRIORS_SOFTMAX
 TERM_MATED = 3                            # terminal code of a game whose side to move has no strictly legal move (strict engines)
 
 _lib = None
@@ -43,6 +44,8 @@ def _sig(L):
     L.cz_engine_leaves.argtypes = [vp]
     L.cz_engine_create_rules.argtypes = [i32, i64, i32, i32, C.POINTER(vp)]
     L.cz_engine_rules.argtypes = [vp]
+    L.cz_engine_set_priors.argtypes = [vp, i32]
+    L.cz_engine_priors.argtypes = [vp]
     L.cz_engine_destroy.argtypes = [vp]
     L.cz_engine_n_games.argtypes = [vp]
     L.cz_engine_reset.argtypes = [vp, vp, vp, vp, vp, vp]

@@ -23,7 +23,7 @@ import torch
 
 from . import rules as _rules                        # (random_openings and Match take a `rules` argument)
 from ._lib import NLABEL, TERM_MATED, EngineError
-from .engine import check_rules
+from .engine import check_priors, check_rules
 from .selfplay import SelfPlay, mt_streams, network_selfplay, sample_moves
 
 NO_MOVE = 0xFFFF
@@ -136,9 +136,10 @@ class MatchResult:
 class _Player:
     """One player's trees of one half of the games: an engine driven by a SelfPlay used for its search() only."""
 
-    def __init__(self, evaluator, n, playouts, search_threads, arena_words, colour, lo, rules="reference"):
+    def __init__(self, evaluator, n, playouts, search_threads, arena_words, colour, lo, rules="reference", priors="reference"):
         self.colour, self.lo, self.hi = colour, lo, lo + n
-        kw = dict(auto_reset=False, keep_records=False, search_threads=search_threads, arena_words=arena_words, rules=rules)
+        kw = dict(auto_reset=False, keep_records=False, search_threads=search_threads, arena_words=arena_words, rules=rules,
+                  priors=priors)
         if hasattr(evaluator, "native_plan"):                       # a policy_value_network: its own plan and precision
             self.sp = network_selfplay(evaluator, n, playouts, **kw)
         else:                                                       # a device callable (nn_in) -> (logits, value)
@@ -151,23 +152,25 @@ class Match:
     """candidate vs best over n_games concurrent games; step() plays one ply of every running game, run() plays them all out."""
 
     def __init__(self, candidate, best, n_games, playouts, search_threads=1, seeds=None, temperature=1e-3, opening_temperature=1.0,
-                 opening_plies=30, openings=None, max_plies=None, arena_words=1 << 20, rules="reference"):
+                 opening_plies=30, openings=None, max_plies=None, arena_words=1 << 20, rules="reference", priors="reference"):
         """rules: 'reference' or 'strict' (every engine searches strictly legal moves only; a side without one is mated and loses;
         needs search_threads = 1; openings should then come from random_openings(..., rules='strict')).  Under strict rules a game
-        whose opening leaves the side to move without a strictly legal move is over before its first ply, won by the other side."""
+        whose opening leaves the side to move without a strictly legal move is over before its first ply, won by the other side.
+        priors: 'reference' or 'softmax', how all four engines turn the networks' logits into priors (Engine priors)."""
         if n_games <= 0 or n_games % 2:
             raise ValueError("n_games must be a positive even number (colour-swapped pairs), got %r" % (n_games,))
         self.rules = check_rules(rules, search_threads)
+        self.priors = check_priors(priors)
         _rules._init_tables()
         self.n, self.half = int(n_games), int(n_games) // 2
         self.temperature, self.opening_temperature, self.opening_plies = temperature, opening_temperature, int(opening_plies)
         self.max_plies = max_plies
         h = self.half
         # players[k]: half k // 2, candidate for even k; the candidate is red ('w') in the first half and black in the second
-        self.players = [_Player(candidate, h, playouts, search_threads, arena_words, 0, 0, self.rules),
-                        _Player(best, h, playouts, search_threads, arena_words, 1, 0, self.rules),
-                        _Player(candidate, h, playouts, search_threads, arena_words, 1, h, self.rules),
-                        _Player(best, h, playouts, search_threads, arena_words, 0, h, self.rules)]
+        self.players = [_Player(candidate, h, playouts, search_threads, arena_words, 0, 0, self.rules, self.priors),
+                        _Player(best, h, playouts, search_threads, arena_words, 1, 0, self.rules, self.priors),
+                        _Player(candidate, h, playouts, search_threads, arena_words, 1, h, self.rules, self.priors),
+                        _Player(best, h, playouts, search_threads, arena_words, 0, h, self.rules, self.priors)]
         self._mt = mt_streams(range(self.n) if seeds is None else seeds)
         if len(self._mt) != self.n:
             raise ValueError("Match: %d seeds for %d games" % (len(self._mt), self.n))
@@ -311,6 +314,8 @@ def main(argv=None):
     ap.add_argument("--search_threads", type=int, default=None, help="default 16 (reference rules) or 1 (strict rules)")
     ap.add_argument("--rules", choices=("reference", "strict"), default="reference",
                     help="strict: both players search strictly legal moves only and a side without one is mated")
+    ap.add_argument("--priors", choices=("reference", "softmax"), default="reference",
+                    help="softmax: the searches use the softmax of the legal moves' logits as priors (reference: logit / sum)")
     ap.add_argument("--res_block_nums", type=int, default=7)
     ap.add_argument("--precision", default="fp16")
     ap.add_argument("--threshold", type=float, default=0.55)
@@ -329,7 +334,7 @@ def main(argv=None):
     openings = random_openings(a.openings, a.opening_moves, a.seed, rules=a.rules) if a.openings > 0 else None
     m = Match(cand, best, a.games, a.playouts, search_threads=threads, seeds=[a.seed + g for g in range(a.games)],
               temperature=a.temperature, opening_temperature=a.opening_temperature, opening_plies=a.opening_plies, openings=openings,
-              max_plies=a.max_plies, rules=a.rules)
+              max_plies=a.max_plies, rules=a.rules, priors=a.priors)
     r = m.run()
     if a.json:
         with open(a.json, "w") as f:

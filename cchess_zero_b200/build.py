@@ -6,7 +6,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = [os.path.join(HERE, "csrc", "cz_engine.cu"), os.path.join(HERE, "csrc", "cz_net.cu"), os.path.join(HERE, "csrc", "cz_tower.cu"),
        os.path.join(HERE, "csrc", "cz_host.cu")]
-DEPS = SRC + [os.path.join(HERE, "csrc", "cz_rules.cuh"), os.path.join(HERE, "csrc", "cz_wgmma.cuh"), os.path.join(os.path.dirname(HERE), "include", "cchess_b200.h")]
+DEPS = SRC + [os.path.join(HERE, "csrc", "cz_rules.cuh"), os.path.join(HERE, "csrc", "cz_wgmma.cuh"), os.path.join(HERE, "csrc", "cz_exp.h"),
+        os.path.join(os.path.dirname(HERE), "include", "cchess_b200.h")]
 LIB = os.path.join(HERE, "libcchess_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--fmad=false",

@@ -40,6 +40,7 @@
 
 #include "../../include/cchess_b200.h"
 #include "cz_rules.cuh"
+#include "cz_exp.h"
 
 #define MAXD 256
 #define NONE 0xFFFFFFFFu
@@ -260,19 +261,45 @@ __device__ int expand_reserve(const Dev &E, WarpSmem &S, uint32_t &alloc, uint32
     alloc = base + size;
     return n;
 }
-// 2: prior gather (lg = this leaf's logits row), serial float32 normalisation, block write
+// Softmax priors (engines with CZ_PRIORS_SOFTMAX, DESIGN 3k): S.ps[0 .. n) holds the gathered logits l_i and receives
+// P_i = f32(e_i / s), e_i = cz_exp(f64(l_i) - f64(m)), m = max l_i with NaNs ignored (fmaxf), s = the f64 sum of the e_i in move
+// order.  Lane l owns children l, l+32, l+64, l+96; the max is a butterfly of fmaxf (exact, any order); every lane adds the e_i in
+// the same serial order from shuffles, so all lanes hold the same s.
+__device__ __forceinline__ void softmax_priors(WarpSmem &S, int n, int lane) {
+    float m = __int_as_float(0x7fffffff);           // NaN: fmaxf's neutral element, and the result when every logit is NaN
+#pragma unroll
+    for (int k = 0; k < 4; k++) { const int i = lane + 32 * k; if (i < n) m = fmaxf(m, S.ps[i]); }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(CZ_FULL, m, o));
+    double e[4];
+#pragma unroll
+    for (int k = 0; k < 4; k++) { const int i = lane + 32 * k; e[k] = i < n ? cz_exp(__dsub_rn((double)S.ps[i], (double)m)) : 0.0; }
+    double s = 0.0;
+#pragma unroll
+    for (int k = 0; k < 4; k++)
+        for (int j = 0; j < 32 && 32 * k + j < n; j++) s = __dadd_rn(s, __shfl_sync(CZ_FULL, e[k], j));
+    __syncwarp();
+#pragma unroll
+    for (int k = 0; k < 4; k++) { const int i = lane + 32 * k; if (i < n) S.ps[i] = __double2float_rn(__ddiv_rn(e[k], s)); }
+    __syncwarp();
+}
+// 2: prior gather (lg = this leaf's logits row), serial float32 normalisation (SOFTMAX: softmax_priors), block write
+template <bool SOFTMAX = false>
 __device__ void expand_write(uint32_t *ar, WarpSmem &S, const float *lg, int n, uint32_t base, int lane, bool with_q = false) {
     for (int i = lane; i < n; i += 32) S.ps[i] = __ldg(lg + S.li[i]);
     __syncwarp();
     const uint32_t cs = (uint32_t)((n + 7) & ~7);
     float tot = 1e-8f;  // tot_p = 1e-8 accumulated in float32, in move order (main.py:176, 184)
+    if constexpr (SOFTMAX) softmax_priors(S, n, lane);
+    else {
 #pragma unroll 8
-    for (int i = 0; i < n; i++) tot = __fadd_rn(tot, S.ps[i]);   // strictly serial adds; unrolled so the LDS latency overlaps
+        for (int i = 0; i < n; i++) tot = __fadd_rn(tot, S.ps[i]);   // strictly serial adds; unrolled so the LDS latency overlaps
+    }
     uint32_t *blk = ar + base;
     if (lane < HDR) blk[lane] = lane == 0 ? (uint32_t)n : 0u;
     for (int i = lane; i < (int)cs; i += 32) {
         const bool live = i < n;
-        blk[HDR + i] = live ? __float_as_uint(__fdiv_rn(S.ps[i], tot)) : 0u;   // n.P /= tot_p (main.py:187)
+        blk[HDR + i] = live ? __float_as_uint(SOFTMAX ? S.ps[i] : __fdiv_rn(S.ps[i], tot)) : 0u;   // n.P /= tot_p (main.py:187)
         blk[HDR + cs + i] = 0u;                                                // W = 0
         blk[HDR + 2 * cs + i] = 0u;                                            // N = 0
         blk[HDR + 3 * cs + i] = live ? (uint32_t)S.moves[i] : 0u;              // META: move, no grandchildren yet
@@ -427,7 +454,8 @@ __device__ __forceinline__ void stage_board(WarpSmem &S, const uint8_t *boards, 
 // block is the bare 8-word header (count 0, linked under its edge with n_grandchildren 0); the playout that expanded it backs up
 // as if the network had returned -1 for the side to move there, and a later descent onto it is a terminal worth +1 to the edge.
 // A game whose root is mated leaves the search.
-template <typename T, bool STRICT>
+// SOFTMAX (engines with CZ_PRIORS_SOFTMAX, likewise in k_wave_multi and k_wave_fifo): expansions write softmax priors (expand_write).
+template <typename T, bool STRICT, bool SOFTMAX>
 __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave(Dev E, T *nn_in, const float *logits, const float *value) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     WarpSmem *smem = reinterpret_cast<WarpSmem *>(smem_raw);
@@ -491,7 +519,7 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave(Dev E, T *nn_in, const
         // ---- round trip 3 (root block of the next descent) is requested BEFORE the logit gather (round trip 4) ----
         if (pend == 1 && done < target) { load_block<false>(ar, root_base, root_cnt, lane, R); have_root = true; }
         if (ok) {
-            expand_write(ar, S, logits + (size_t)g * CZ_NLABEL, n, base, lane);
+            expand_write<SOFTMAX>(ar, S, logits + (size_t)g * CZ_NLABEL, n, base, lane);
             if (pend == 2) { root_base = base; root_cnt = n; }
             else {
                 uint2 last;
@@ -626,7 +654,7 @@ __constant__ uint8_t c_start[96];   // start position, uploaded by cz_engine_cre
 // currently hold a virtual loss on it (META bits 24-30) so that Q is taken from the loss-free statistics like the reference's
 // stale Q (main.py:403-404 never touches Q); an unexpanded child that is already being evaluated is `claimed` (bit 31) and a
 // second descent that reaches it backs off (the reference waits on now_expanding, main.py:354-355).
-template <typename T>
+template <typename T, bool SOFTMAX>
 __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave_multi(Dev E, T *nn_in, const float *logits, const float *value) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     WarpSmem *smem = reinterpret_cast<WarpSmem *>(smem_raw);
@@ -664,7 +692,7 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave_multi(Dev E, T *nn_in,
         const int n = expand_reserve<false>(E, S, alloc, base, errf, lane);
         const bool ok = n > 0;
         if (ok) {
-            expand_write(ar, S, logits + idx * CZ_NLABEL, n, base, lane);
+            expand_write<SOFTMAX>(ar, S, logits + idx * CZ_NLABEL, n, base, lane);
             if (pend == 2) { root_base = base; root_cnt = n; }
             else if (lane == 0) expand_link(ar, path[depth - 1], n, base, 1u);    // exactly one playout (ours) holds a loss on a claimed edge
             if (lane == 0) { atomicAdd(E.cnt_expand + g, 1ull); atomicAdd(E.cnt_C + g, (unsigned long long)n); }
@@ -812,7 +840,7 @@ __device__ void warp_unwind_q(const uint2 *path, uint32_t *ar, int depth, float 
     __syncwarp();
 }
 
-template <typename T>
+template <typename T, bool SOFTMAX>
 __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave_fifo(Dev E, T *nn_in, const float *logits, const float *value) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     WarpSmem *smem = reinterpret_cast<WarpSmem *>(smem_raw);
@@ -859,7 +887,7 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave_fifo(Dev E, T *nn_in, 
         uint32_t base;
         const int n = expand_reserve<false>(E, S, alloc, base, errf, lane);
         if (n > 0) {
-            expand_write(ar, S, logits + NN_ROW((size_t)g * K) * CZ_NLABEL, n, base, lane, true);
+            expand_write<SOFTMAX>(ar, S, logits + NN_ROW((size_t)g * K) * CZ_NLABEL, n, base, lane, true);
             root_base = base; root_cnt = n;
             if (lane == 0) { atomicAdd(E.cnt_expand + g, 1ull); atomicAdd(E.cnt_C + g, (unsigned long long)n); }
         } else { flags &= ~F_ACTIVE; dead = true; }
@@ -896,7 +924,7 @@ __global__ void __launch_bounds__(32 * MAX_WPB, 1) k_wave_fifo(Dev E, T *nn_in, 
                     uint32_t base;
                     const int n = expand_reserve<false>(E, S, alloc, base, errf, lane);
                     if (n > 0) {
-                        expand_write(ar, S, logits + NN_ROW(idx) * CZ_NLABEL, n, base, lane, true);
+                        expand_write<SOFTMAX>(ar, S, logits + NN_ROW(idx) * CZ_NLABEL, n, base, lane, true);
                         if (lane == 0) {
                             expand_link(ar, path[plen - 1], n, base, 0u);               // also clears `claimed`: now_expanding.remove(node)
                             atomicAdd(E.cnt_expand + g, 1ull); atomicAdd(E.cnt_C + g, (unsigned long long)n);
@@ -1627,6 +1655,8 @@ struct cz_engine {
     uint32_t *d_snap = nullptr;      // device staging of snapshot blobs, grown on demand
     size_t snap_cap = 0;
     int rules = CZ_RULES_REFERENCE;  // CZ_RULES_STRICT: k_wave<T, true>, k_play_moves<true> and k_root_mate after every root change
+    int priors = CZ_PRIORS_REFERENCE;  // CZ_PRIORS_SOFTMAX: the wave kernels' SOFTMAX instantiations
+    bool waved = false;                // a wave has been launched: the prior mode is fixed
 };
 
 extern "C" {
@@ -1892,6 +1922,15 @@ int cz_engine_create_rules(int n_games, int64_t arena_words, int device, int rul
     return rc;
 }
 int cz_engine_rules(const cz_engine *e) { return e ? e->rules : CZ_EINVAL; }
+int cz_engine_set_priors(cz_engine *e, int mode) {
+    if (!e) return fail(CZ_EINVAL, "cz_engine_set_priors: null engine");
+    if (mode != CZ_PRIORS_REFERENCE && mode != CZ_PRIORS_SOFTMAX)
+        return fail(CZ_EINVAL, "cz_engine_set_priors: mode must be CZ_PRIORS_REFERENCE or CZ_PRIORS_SOFTMAX");
+    if (e->waved) return fail(CZ_EINVAL, "cz_engine_set_priors: the engine has already run a wave");
+    e->priors = mode;
+    return CZ_OK;
+}
+int cz_engine_priors(const cz_engine *e) { return e ? e->priors : CZ_EINVAL; }
 
 extern "C++" {
 static int create_engine(int n_games, int64_t arena_words, int device, int leaves, bool fifo, cz_engine **out) {
@@ -2040,12 +2079,21 @@ int cz_engine_wave(cz_engine *e, void *stream, void *nn_in, int nn_dtype, const 
     dim3 gr(nblk(e->d.B, e->wpb)), bl(32 * e->wpb);
     const size_t sm = (size_t)e->wpb * sizeof(WarpSmem);
     cudaStream_t st = (cudaStream_t)stream;
+    e->waved = true;
+    const bool softmax = e->priors == CZ_PRIORS_SOFTMAX;
     return launch_nn_typed(nn_dtype, nn_in, [&](auto *in) {
         using T = std::remove_pointer_t<decltype(in)>;
-        if (e->d.fifo) k_wave_fifo<T><<<gr, bl, sm, st>>>(e->d, in, logits, value);          // search_threads = K schedule of the reference
-        else if (e->d.pendK) k_wave_multi<T><<<gr, bl, sm, st>>>(e->d, in, logits, value);   // leaf-parallel engine
-        else if (e->rules == CZ_RULES_STRICT) k_wave<T, true><<<gr, bl, sm, st>>>(e->d, in, logits, value);
-        else k_wave<T, false><<<gr, bl, sm, st>>>(e->d, in, logits, value);
+        if (softmax) {
+            if (e->d.fifo) k_wave_fifo<T, true><<<gr, bl, sm, st>>>(e->d, in, logits, value);
+            else if (e->d.pendK) k_wave_multi<T, true><<<gr, bl, sm, st>>>(e->d, in, logits, value);
+            else if (e->rules == CZ_RULES_STRICT) k_wave<T, true, true><<<gr, bl, sm, st>>>(e->d, in, logits, value);
+            else k_wave<T, false, true><<<gr, bl, sm, st>>>(e->d, in, logits, value);
+        } else {
+            if (e->d.fifo) k_wave_fifo<T, false><<<gr, bl, sm, st>>>(e->d, in, logits, value);          // search_threads = K schedule of the reference
+            else if (e->d.pendK) k_wave_multi<T, false><<<gr, bl, sm, st>>>(e->d, in, logits, value);   // leaf-parallel engine
+            else if (e->rules == CZ_RULES_STRICT) k_wave<T, true, false><<<gr, bl, sm, st>>>(e->d, in, logits, value);
+            else k_wave<T, false, false><<<gr, bl, sm, st>>>(e->d, in, logits, value);
+        }
     });
 }
 // search_threads = K engines: one wave with row compaction.  nn_stage [B*K rows] receives every slot's input row as cz_engine_wave

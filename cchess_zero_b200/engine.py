@@ -8,7 +8,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import BF16, BOARD, F16, F32, MAXCHILD, RULES, STATUS_BYTES, EngineError, check, lib
+from ._lib import BF16, BOARD, F16, F32, MAXCHILD, PRIORS, RULES, STATUS_BYTES, EngineError, check, lib
 
 _DT = {torch.float32: F32, torch.bfloat16: BF16, torch.float16: F16, torch.uint8: BOARD}
 
@@ -32,16 +32,27 @@ def check_rules(rules, search_threads=1, leaves=1):
     return rules
 
 
+def check_priors(priors):
+    """The prior mode `priors` names: 'reference' (P = logit / (1e-8 + the sum of the legal logits), the reference's expansion) or
+    'softmax' (P = the softmax of the legal logits, DESIGN 3k); ValueError for another name.  Every engine kind takes either."""
+    if priors not in PRIORS:
+        raise ValueError("priors must be 'reference' or 'softmax', not %r" % (priors,))
+    return priors
+
+
 class Engine:
-    def __init__(self, n_games, arena_words=0, device=None, leaves=1, search_threads=None, rules="reference"):
+    def __init__(self, n_games, arena_words=0, device=None, leaves=1, search_threads=None, rules="reference", priors="reference"):
         """leaves > 1: leaf-parallel engine (up to `leaves` leaves per game per wave; network rows = n_games*leaves).
         leaves == -1: the leaf-parallel kernel with one slot (test hook).
         search_threads = K: the reference's search_threads schedule in canonical FIFO form (bit-exact with the reference's
         uvloop runs wherever those are reproducible); network rows = n_games*K.
         rules: 'reference' (pseudo-legal moves, a game ends when a king is taken) or 'strict' (strictly legal moves only; a side
         without one is mated, terminal code 3; cz_engine_create_rules).  Strict rules need the one-leaf engine: no search_threads
-        (any search_threads value, 1 included, builds the FIFO engine) and leaves = 1."""
+        (any search_threads value, 1 included, builds the FIFO engine) and leaves = 1.
+        priors: 'reference' or 'softmax', how an expansion turns the network's logits into priors (check_priors;
+        cz_engine_set_priors before the first wave)."""
         check_rules(rules, 1, leaves)
+        check_priors(priors)
         if rules == "strict" and search_threads is not None:
             raise ValueError("strict rules need the one-leaf engine: search_threads = %r builds the search_threads schedule's (FIFO) "
                              "engine, which plays by the reference rules; leave search_threads unset" % (search_threads,))
@@ -61,6 +72,9 @@ class Engine:
         else:
             check(lib().cz_engine_create_ex(self.B, int(arena_words), self.device, int(leaves), C.byref(h)), "cz_engine_create_ex")
         self.h = h
+        self.priors = priors
+        if priors != "reference":
+            check(lib().cz_engine_set_priors(h, PRIORS[priors]), "cz_engine_set_priors")
         self.launches = 0   # kernels of csrc/cz_engine.cu launched through this handle
         self._mate = 1 if rules == "strict" else 0          # k_root_mate after every root change of a strict engine
         self._count = torch.zeros(1, dtype=torch.int32, device="cuda:%d" % self.device)

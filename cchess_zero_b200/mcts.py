@@ -55,7 +55,7 @@ class _Root(object):
 
 
 class MCTS_tree(object):
-    def __init__(self, in_state, in_forward, search_threads, arena_words=1 << 21, leaf_parallel=1):
+    def __init__(self, in_state, in_forward, search_threads, arena_words=1 << 21, leaf_parallel=1, priors="reference"):
         """leaf_parallel = K > 1 evaluates up to K leaves of this tree per network call (virtual-loss batching; faster moves,
         deterministic, but no longer the reference's search_threads=1 visit counts).  Default 1 = bit-exact mode."""
         self.noise_eps = 0.25
@@ -71,7 +71,9 @@ class MCTS_tree(object):
         if self.fifo and int(search_threads) > 32:
             raise ValueError("search_threads > 32 is not supported by the device event loop")
         self.K = int(search_threads) if self.fifo else max(1, int(leaf_parallel))
-        self.engine = Engine(1, arena_words, search_threads=self.K) if self.fifo else Engine(1, arena_words, leaves=self.K)
+        # priors: 'reference' (logit / sum, the reference's expansion) or 'softmax' (Engine priors)
+        self.engine = (Engine(1, arena_words, search_threads=self.K, priors=priors) if self.fifo
+                       else Engine(1, arena_words, leaves=self.K, priors=priors))
         dev = torch.device("cuda", self.engine.device)
         owner = getattr(in_forward, "__self__", None)
         K = self.K

@@ -13,7 +13,8 @@ class ChessGame(object):
     """Text-mode stand-in for the reference's ChessGame: same constructor arguments, start()/perform_AI()/change_player()."""
 
     def __init__(self, in_ai_count, in_ai_function, in_play_playout, in_delay=0.0, in_end_delay=0.0, batch_size=128, search_threads=16,
-                 processor="gpu", num_gpus=1, res_block_nums=7, human_color="b", network=None, quiet=False, strict=False):
+                 processor="gpu", num_gpus=1, res_block_nums=7, human_color="b", network=None, quiet=False, strict=False,
+                 priors="reference"):
         self.ai_count, self.ai_function = in_ai_count, in_ai_function
         self.delay, self.end_delay, self.quiet = in_delay, in_end_delay, quiet
         self.current_player = "w"
@@ -21,7 +22,7 @@ class ChessGame(object):
         self.move_times = []
         self.cchess_engine = cchess_main(playout=in_play_playout, in_batch_size=batch_size, exploration=False, in_search_threads=search_threads,
                                          processor=processor, num_gpus=num_gpus, res_block_nums=res_block_nums, human_color=human_color,
-                                         network=network, log_file=False, strict=strict)
+                                         network=network, log_file=False, strict=strict, priors=priors)
 
     def perform_AI(self):  # ChessGame.py:183-195
         t0 = time.perf_counter()
@@ -63,9 +64,12 @@ def main():
     ap.add_argument("--delay", default=0.0, type=float)
     ap.add_argument("--res_block_nums", default=7, type=int)
     ap.add_argument("--human_color", default="b", choices=["w", "b"])
+    ap.add_argument("--priors", default="reference", choices=["reference", "softmax"],
+                    help="softmax: the AI searches (and, with --ai_function net, ranks moves) by the softmax of the legal moves' logits")
     a = ap.parse_args()
     # a human at the terminal expects the full rules: no self-check, mate ends the game
-    g = ChessGame(a.ai_count, a.ai_function, a.play_playout, a.delay, res_block_nums=a.res_block_nums, human_color=a.human_color, strict=True)
+    g = ChessGame(a.ai_count, a.ai_function, a.play_playout, a.delay, res_block_nums=a.res_block_nums, human_color=a.human_color, strict=True,
+                  priors=a.priors)
     print("result:", g.start())
 
 

@@ -20,7 +20,7 @@ import torch
 
 from . import rules as _rules                        # (SelfPlay takes a `rules` argument)
 from ._lib import MAXCHILD, MT_WORDS, NLABEL, NSQ, TERM_MATED, EngineError, lib
-from .engine import Engine, capture_cuda_graph, check_rules, run_waves
+from .engine import Engine, capture_cuda_graph, check_priors, check_rules, run_waves
 
 
 def _vp(a):
@@ -252,16 +252,20 @@ class SelfPlay:
     def __init__(self, n_games, forward, playouts, seeds=None, exploration=True, temperature=1,
                  nn_dtype=torch.float32, arena_words=0, auto_reset=True, device=None, keep_records=True, plan=None,
                  plan_factory=None, lanes=1, engine=None, hashing=False, search_threads=1, compact=None, rules="reference",
-                 root_noise=None):
+                 root_noise=None, priors="reference"):
         """plan: an InferencePlan / NativePlan (defines the input buffer, writes logits/value in place); plan_factory(rows) builds
         one when `plan` is not given.  lanes: 1 is the only value.  rules: 'reference' or 'strict' (the search expands strictly legal
         moves only and a side without one is mated: the game ends with terminal code 3, won by the side that moved last); strict
         rules need search_threads = 1.  root_noise: None (off) or (eps, alpha): every search() first mixes Dirichlet noise into the
-        root priors of its games, P' = (1 - eps) P + eps Dir(alpha) (see search)."""
+        root priors of its games, P' = (1 - eps) P + eps Dir(alpha) (see search).  priors: 'reference' or 'softmax', how the search
+        turns the network's logits into priors (Engine priors; the noise mixes into either)."""
         if lanes != 1:
             raise ValueError("SelfPlay: lanes must be 1")
         self.rules = check_rules(rules, search_threads)
         self.root_noise = check_root_noise(root_noise)
+        self.priors = check_priors(priors)
+        if engine is not None and getattr(engine, "priors", "reference") != priors:
+            raise ValueError("SelfPlay: the engine uses the %r priors, not %r" % (getattr(engine, "priors", "reference"), priors))
         if engine is not None and getattr(engine, "rules", "reference") != rules:
             raise ValueError("SelfPlay: the engine plays by the %r rules, not %r" % (getattr(engine, "rules", "reference"), rules))
         self.B = n_games
@@ -272,8 +276,8 @@ class SelfPlay:
         assert not self.compact or self.K > 1, "row compaction belongs to the search_threads = K engine"
         # `engine`: an object with the Engine interface (tests drive the host loop with a CPU stand-in); the product
         # always constructs the CUDA engine here
-        self.engine = engine if engine is not None else (Engine(n_games, arena_words, device, search_threads=self.K) if self.K > 1
-                                                         else Engine(n_games, arena_words, device, rules=rules))
+        self.engine = engine if engine is not None else (Engine(n_games, arena_words, device, search_threads=self.K, priors=priors)
+                                                         if self.K > 1 else Engine(n_games, arena_words, device, rules=rules, priors=priors))
         if hashing:                              # Zobrist keys of the pending leaves (must be on before a graph is captured)
             self.engine.enable_hashing(True)
         dev = torch.device("cuda", self.engine.device) if engine is None else torch.device(getattr(engine, "torch_device", "cpu"))
@@ -505,7 +509,7 @@ class SelfPlay:
     def save_games(self, path):
         """Every game in flight into one np.savez file (written to a temporary file, then renamed): the engine's trees and game state
         (Engine.snapshot) and the host state -- boards, sides, live, the per-slot MT19937 states (and, with root noise, the noise
-        streams' states under 'noise_mt'), plies, temperature and each slot's unfinished record (its players and log span).  load_games
+        streams' states under 'noise_mt'; with softmax priors, priors='softmax'), plies, temperature and each slot's unfinished record (its players and log span).  load_games
         continues exactly where this left off.  The finished games must have been handed over with pop_finished first."""
         if self.finished:
             raise ValueError("save_games: %d finished games were not drained with pop_finished()" % len(self.finished))
@@ -516,6 +520,8 @@ class SelfPlay:
         players = [self.records[g].players for g in range(self.B)]
         if self.root_noise is not None:
             log["noise_mt"] = self._noise_mt
+        if self.priors != "reference":                                 # (absent: reference priors, so older files stay as they were)
+            log["priors"] = np.asarray(self.priors)
         _savez(path, engine=blob, boards=self.boards, sides=self.sides, live=self.live, mt=self._mt, plies=np.int64(self.plies),
                temperature=np.asarray(self.temperature, dtype=np.float64), span_len=np.asarray([len(s) for s in self._span], dtype=np.int64),
                players_len=np.asarray([len(p) for p in players], dtype=np.int64),
@@ -523,7 +529,7 @@ class SelfPlay:
 
     def load_games(self, path):
         """Restore what save_games wrote into this SelfPlay (same number of games and engine kind, root noise on in both or in neither;
-        the engine is restored in place, so a captured graph stays valid).  The file is read without pickle and checked; ValueError / EngineError leave everything as it
+        the same prior mode; the engine is restored in place, so a captured graph stays valid).  The file is read without pickle and checked; ValueError / EngineError leave everything as it
         was."""
         with np.load(path, allow_pickle=False) as d:
             a = {k: d[k] for k in d.files}
@@ -537,6 +543,9 @@ class SelfPlay:
         if ("noise_mt" in a) != (self.root_noise is not None):        # the noise streams are part of an exact resume
             raise ValueError("games file: saved %s root noise, this SelfPlay runs %s" % (("with", "without") if "noise_mt" in a
                                                                                         else ("without", "with")))
+        saved = str(a["priors"]) if "priors" in a else "reference"
+        if saved != self.priors:                                       # the trees were searched with the saved file's priors
+            raise ValueError("games file: saved with %r priors, this SelfPlay uses %r" % (saved, self.priors))
         if self.root_noise is not None:
             want["noise_mt"] = ((B, MT_WORDS), np.uint32)
         for k, (shp, dt) in want.items():
@@ -585,6 +594,20 @@ class SelfPlay:
         return sorted(self.finished, key=lambda t: t[0])
 
 
+def softmax_priors(logits):
+    """The softmax priors of one node's legal-move logits (float32, in move order), as the engine computes them with
+    priors='softmax' (DESIGN 3k) up to the last bit of the exponential: m = the largest logit (NaNs ignored), e_i = exp(f64(l_i) - m),
+    s = the serial f64 sum of the e_i, P_i = f32(e_i / s).  float32 array."""
+    lg = np.asarray(logits, dtype=np.float32).astype(np.float64)
+    if lg.size == 0:
+        return np.zeros(0, dtype=np.float32)
+    e = np.exp(lg - np.fmax.reduce(lg))
+    s = 0.0
+    for v in e:
+        s += v
+    return (e / s).astype(np.float32)
+
+
 def network_selfplay(network, n_games, playouts, **kw):
     """SelfPlay evaluated by a policy_value_network: an fp16 network runs its native plan (board bytes in, the hand-written first
     convolution and heads), any other precision its own inference plan.  Either plan follows the network's weights_version, so a
@@ -628,7 +651,8 @@ class cchess_main(object):
     banned_moves = ()       # move labels the next get_action / select_move must not play (a GUI's perpetual-check ban)
 
     def __init__(self, playout=400, in_batch_size=128, exploration=True, in_search_threads=16, processor="cpu",
-                 num_gpus=1, res_block_nums=7, human_color="b", network=None, log_file=True, leaf_parallel=1, strict=False):
+                 num_gpus=1, res_block_nums=7, human_color="b", network=None, log_file=True, leaf_parallel=1, strict=False,
+                 priors="reference"):
         from .mcts import MCTS_tree
         from .net import policy_value_network, policy_value_network_gpus
         _rules._init_tables()
@@ -650,7 +674,10 @@ class cchess_main(object):
         else:  # `processor` selected CPU/GPU TensorFlow in the reference (main.py:1142); both map to the CUDA net here
             self.policy_value_netowrk = policy_value_network(res_block_nums) if processor == "cpu" else policy_value_network_gpus(num_gpus, res_block_nums)
         self.search_threads = in_search_threads
-        self.mcts = MCTS_tree(self.game_borad.state, self.policy_value_netowrk.forward, self.search_threads, leaf_parallel=leaf_parallel)
+        # priors='softmax': the search and the 'net' player use the softmax of the legal moves' logits (reference: logit / sum)
+        self.priors = check_priors(priors)
+        self.mcts = MCTS_tree(self.game_borad.state, self.policy_value_netowrk.forward, self.search_threads, leaf_parallel=leaf_parallel,
+                              priors=priors)
         self.exploration = exploration
         self.resign_threshold = -0.8
         self.global_step = 0
@@ -754,6 +781,8 @@ class cchess_main(object):
             action_probs = cchess_main.flip_policy(action_probs)
         moves = _rules.GameBoard.get_legal_moves(self.game_borad.state, self.game_borad.current_player)
         action_probs = np.asarray(action_probs).flatten()
+        if getattr(self, "priors", "reference") == "softmax":
+            return moves, list(softmax_priors(action_probs[[_rules.label2i[a] for a in moves]])), value
         tot_p = 1e-8
         p = []
         for action in moves:
@@ -916,10 +945,11 @@ class cchess_main(object):
         """Plays n_games (even: colour-swapped pairs) of this network against `opponent` (another policy_value_network; None = a
         search-only opponent with zero logits and zero value -- the reference's stub used pure MCTS with random rollouts, which
         this engine does not have), self.playout_counts playouts per move and self.search_threads, all games at once
-        (arena.Match).  Prints the stub's line and returns win_ratio = (win + 0.5 tie) / n_games."""
+        (arena.Match, both sides searching with this instance's priors).  Prints the stub's line and returns win_ratio = (win + 0.5 tie)
+        / n_games."""
         from .arena import Match, UniformEvaluator
         r = Match(self.policy_value_netowrk, UniformEvaluator() if opponent is None else opponent, n_games, self.playout_counts,
-                  search_threads=self.search_threads).run()
+                  search_threads=self.search_threads, priors=getattr(self, "priors", "reference")).run()
         win_ratio = 1.0 * (r.wins + 0.5 * r.draws) / n_games
         print("num_playouts:{}, win: {}, lose: {}, tie:{}".format(self.playout_counts, r.wins, r.losses, r.draws))
         return win_ratio
@@ -927,9 +957,10 @@ class cchess_main(object):
     # ---- batched bridge: many games at once on this rank's GPU ---------------------------------------
     def selfplay_many(self, n_games, seeds=None, arena_words=0):
         """Plays n_games concurrent games with the engine's lock-step waves and returns a list of
-        (zip(states, mcts_probs, z), n) -- the same tuples selfplay() yields, one entry per game."""
+        (zip(states, mcts_probs, z), n) -- the same tuples selfplay() yields, one entry per game.  The games search with this instance's
+        priors."""
         net = self.policy_value_netowrk
         plan = net.plan()
         sp = SelfPlay(n_games, None, self.playout_counts, seeds=seeds, exploration=self.exploration, temperature=self.temperature,
-                      arena_words=arena_words, auto_reset=False, plan=plan)
+                      arena_words=arena_words, auto_reset=False, plan=plan, priors=getattr(self, "priors", "reference"))
         return [(rec.tuples(), len(rec)) for _, rec in sp.play_games()]

@@ -281,22 +281,26 @@ class Trainer:
     save(dir) / load(dir) keep everything a run needs to continue: the network(s) with their optimizer state, the replay buffer,
     the sampler's random state, every game slot's MT19937 states (move choice and, with root noise, the noise stream), lr_multiplier,
     the counters and the games in flight (SelfPlay.save_games: the engine's trees and each slot's unfinished record), so a resumed
-    run plays on exactly as the uninterrupted one.  load refuses a run saved with other rules or another root noise setting.  A directory saved without games.npz resumes with fresh games in every slot (drawing from the restored
+    run plays on exactly as the uninterrupted one.  load refuses a run saved with other rules, another root noise setting or
+    other priors.  A directory saved without games.npz resumes with fresh games in every slot (drawing from the restored
     per-slot streams)."""
 
     def __init__(self, network, n_games, playouts, search_threads=1, batch_size=512, buffer_size=10000, epochs=5, kl_targ=0.025,
                  learning_rate=1e-3, updates_per_game=1, mirror=False, eval_every=0, eval_games=10, eval_playouts=None,
-                 gate_threshold=0.55, checkpoint_every=100, seed=0, arena_words=1 << 20, best=None, rules="reference", root_noise=None):
+                 gate_threshold=0.55, checkpoint_every=100, seed=0, arena_words=1 << 20, best=None, rules="reference", root_noise=None,
+                 priors="reference"):
         """rules: 'reference' or 'strict' -- self-play and the gate's matches search strictly legal moves only and a side without
         one is mated (the network learns the full rules of xiangqi); strict rules need search_threads = 1.  root_noise: None or
         (eps, alpha) -- Dirichlet noise on the root priors of every self-play search (SelfPlay root_noise); the gate's matches
-        stay noise-free."""
-        from .engine import check_rules
+        stay noise-free.  priors: 'reference' or 'softmax' -- how self-play and the gate's matches turn the network's logits into
+        priors (SelfPlay priors)."""
+        from .engine import check_priors, check_rules
         from .selfplay import check_root_noise, network_selfplay
         if eval_every and (eval_games <= 0 or eval_games % 2):
             raise ValueError("eval_games must be a positive even number (colour-swapped pairs)")
         self.rules = check_rules(rules, search_threads)
         self.root_noise = check_root_noise(root_noise)
+        self.priors = check_priors(priors)
         self.network = network
         self.n_games, self.playouts, self.search_threads = int(n_games), playouts, int(search_threads)
         self.batch_size, self.epochs, self.kl_targ = int(batch_size), int(epochs), kl_targ
@@ -313,7 +317,7 @@ class Trainer:
         self.buffer = ReplayBuffer(buffer_size, network.device.index)
         self.sp = network_selfplay(self.best or network, self.n_games, playouts, seeds=[self.seed * self.n_games + g for g in range(self.n_games)],
                                    search_threads=self.search_threads, arena_words=arena_words, auto_reset=True, keep_records=True,
-                                   rules=self.rules, root_noise=self.root_noise)
+                                   rules=self.rules, root_noise=self.root_noise, priors=self.priors)
         self.sp.capture_graph()
         self.games = self.positions = self.updates = self.train_steps = self.promotions = self.gates = self.plies = 0
         self.next_gate = self.eval_every
@@ -363,7 +367,8 @@ class Trainer:
         from .arena import Match
         g0 = self.gates * self.eval_games
         r = Match(self.network, self.best, self.eval_games, self.eval_playouts, search_threads=self.search_threads,
-                  seeds=range(g0, g0 + self.eval_games), arena_words=self.arena_words, rules=self.rules).run()
+                  seeds=range(g0, g0 + self.eval_games), arena_words=self.arena_words, rules=self.rules,
+                  priors=self.priors).run()
         self.gates += 1
         self.last_gate = json.loads(r.to_json(self.gate_threshold, games=False))
         if r.promote(self.gate_threshold):
@@ -442,6 +447,9 @@ class Trainer:
         noise = dict(root_noise=np.asarray(self.root_noise or (), dtype=np.float64))
         if self.root_noise is not None:
             noise["noise_mt"] = self.sp._noise_mt
+        priors = getattr(self, "priors", "reference")
+        if priors != "reference":                          # (absent: reference priors, so the default run's file is unchanged)
+            noise["priors"] = np.asarray(priors)
         _savez(os.path.join(directory, "trainer.npz"), rng_version=version, rng_internal=np.asarray(internal, dtype=np.uint32),
                rng_gauss=np.float64(0.0 if gauss is None else gauss), rng_has_gauss=gauss is not None, mt=self.sp._mt, **noise,
                lr_multiplier=self.lr_multiplier, next_gate=self.next_gate, rules=np.asarray(self.rules),
@@ -461,6 +469,9 @@ class Trainer:
             saved = tuple(float(v) for v in rn) if rn.size else None
             if saved != self.root_noise:
                 raise ValueError("saved run has root noise %r, this Trainer %r" % (saved, self.root_noise))
+            saved, priors = (str(d["priors"]) if "priors" in d.files else "reference"), getattr(self, "priors", "reference")
+            if saved != priors:
+                raise ValueError("saved run uses the %r priors, this Trainer %r" % (saved, priors))
             noise_mt = d["noise_mt"].copy() if self.root_noise is not None else None
             gauss = float(d["rng_gauss"]) if bool(d["rng_has_gauss"]) else None
             self.rng.setstate((int(d["rng_version"]), tuple(int(v) for v in d["rng_internal"]), gauss))
@@ -507,6 +518,9 @@ def main(argv=None):
                     help="strict: search strictly legal moves only; a side without one is mated (needs --search-threads 1)")
     ap.add_argument("--root-noise", nargs=2, type=float, metavar=("EPS", "ALPHA"), default=None,
                     help="Dirichlet noise on the self-play root priors: P' = (1 - EPS) P + EPS Dir(ALPHA), e.g. 0.25 0.3")
+    ap.add_argument("--priors", choices=("reference", "softmax"), default="reference",
+                    help="softmax: self-play and the gate search with the softmax of the legal moves' logits as priors (reference: "
+                         "logit / sum, the reference's expansion)")
     a = ap.parse_args(argv)
     from .net import policy_value_network
     out = sys.stdout
@@ -517,7 +531,8 @@ def main(argv=None):
         t = Trainer(net, a.games, a.playouts, search_threads=a.search_threads, batch_size=a.batch_size, buffer_size=a.buffer_size,
                     epochs=a.epochs, learning_rate=a.learning_rate, updates_per_game=a.updates_per_game, mirror=a.mirror,
                     eval_every=a.eval_every, eval_games=a.eval_games, eval_playouts=a.eval_playouts, gate_threshold=a.gate_threshold,
-                    checkpoint_every=a.checkpoint_every, seed=a.seed, rules=a.rules, root_noise=a.root_noise)
+                    checkpoint_every=a.checkpoint_every, seed=a.seed, rules=a.rules, root_noise=a.root_noise,
+                    priors=a.priors)
         if t.best is not None:
             t.best.save_dir = os.path.join(a.save_dir, "best")
         if a.resume and os.path.isfile(os.path.join(a.save_dir, "trainer.npz")):

@@ -3,7 +3,7 @@ Universal Chinese Chess Interface text protocol instead of the reference's tkint
 
     python -m cchess_zero_b200.ucci [--playouts 1200] [--res_block_nums 7] [--leaf_parallel 8]
 
-Commands understood: ucci, isready, setoption name <playouts|leaf_parallel|temperature> value <v>, position {startpos | fen <fen>}
+Commands understood: ucci, isready, setoption name <playouts|leaf_parallel|temperature|priors> value <v>, position {startpos | fen <fen>}
 [moves m1 m2 ...], banmoves m1 m2 ... (the next go does not play them; the next position clears them), go [nodes N | depth D | time ms ...] (nodes = playouts; depth/time are accepted and
 ignored -- the reference searches a fixed playout count, main.py:1336), stop (no-op: go is synchronous like the reference's
 blocking forward), probe/d (print position), quit.
@@ -17,6 +17,8 @@ The search object is injected (`driver`): anything with cchess_main's attributes
 one with strict=True: it never answers with a move that leaves its own king attacked, and answers nobestmove when it is mated.
 main() also checks the moves of `position` for strict legality (`legal_moves`) and refuses a list that holds an illegal one."""
 import sys
+
+from ._lib import PRIORS
 
 START_STATE = "RNBAKABNR/9/1C5C1/P1P1P1P1P/9/9/p1p1p1p1p/1c5c1/9/rnbakabnr"
 START_FEN = "rnbakabnr/9/1c5c1/p1p1p1p1p/9/9/P1P1P1P1P/1C5C1/9/RNBAKABNR w - - 0 1"
@@ -107,14 +109,17 @@ class UcciEngine:
 
     NAME = "cchess-zero-b200"
 
-    def __init__(self, driver_factory, out=None, playouts=1200, leaf_parallel=1, legal_moves=None):
+    def __init__(self, driver_factory, out=None, playouts=1200, leaf_parallel=1, legal_moves=None, priors="reference"):
         """legal_moves: (state, player) -> [move labels]; when given, every move of a `position` command must be in it."""
         self._factory = driver_factory
         self._legal_moves = legal_moves
         self._banned = ()
         self._driver = None
         self.out = out if out is not None else sys.stdout
-        self.options = {"playouts": int(playouts), "leaf_parallel": int(leaf_parallel), "temperature": 1e-3}
+        self.options = {"playouts": int(playouts), "leaf_parallel": int(leaf_parallel), "temperature": 1e-3,
+                        "priors": priors}
+        if priors not in PRIORS:
+            raise ValueError("priors must be 'reference' or 'softmax', not %r" % (priors,))
         self._base = (START_STATE, "w", 0)
         self._moves = ()
         self._synced = None          # (base, moves) the driver's tree currently stands on
@@ -172,6 +177,7 @@ class UcciEngine:
         self._say("option playouts type spin min 1 max 1000000 default %d" % self.options["playouts"])
         self._say("option leaf_parallel type spin min 1 max 16 default %d" % self.options["leaf_parallel"])
         self._say("option temperature type string default %g" % self.options["temperature"])
+        self._say("option priors type combo default %s var reference var softmax" % self.options["priors"])
         self._say("ucciok")
 
     def cmd_isready(self, args):
@@ -187,9 +193,15 @@ class UcciEngine:
         if key not in self.options:
             self._say("info string unknown option %s" % a[0])
             return
-        self.options[key] = float(a[1]) if key == "temperature" else int(a[1])
-        if key == "leaf_parallel" and self._driver is not None:
-            self._driver = None      # K is a construction-time property of the engine handle (cz_engine_create_ex)
+        if key == "priors":
+            if a[1] not in PRIORS:
+                self._say("info string priors must be reference or softmax, not %s" % a[1])
+                return
+            self.options[key] = a[1]
+        else:
+            self.options[key] = float(a[1]) if key == "temperature" else int(a[1])
+        if key in ("leaf_parallel", "priors") and self._driver is not None:
+            self._driver = None      # K and the priors are construction-time properties of the engine handle
         elif key == "playouts" and self._driver is not None:
             self._driver.playout_counts = self.options["playouts"]
 
@@ -290,7 +302,7 @@ def _real_driver(res_block_nums):
     def make(options):
         from .selfplay import cchess_main
         return cchess_main(playout=options["playouts"], exploration=False, processor="gpu", res_block_nums=res_block_nums,
-                           log_file=False, leaf_parallel=options["leaf_parallel"], strict=True)
+                           log_file=False, leaf_parallel=options["leaf_parallel"], strict=True, priors=options["priors"])
     return make
 
 
@@ -301,10 +313,12 @@ def main():
     ap.add_argument("--playouts", default=1200, type=int)
     ap.add_argument("--leaf_parallel", default=8, type=int)
     ap.add_argument("--res_block_nums", default=7, type=int)
+    ap.add_argument("--priors", default="reference", choices=("reference", "softmax"),
+                    help="softmax: search with the softmax of the legal moves' logits as priors (reference: logit / sum)")
     a = ap.parse_args()
     from .rules import GameBoard
     eng = UcciEngine(_real_driver(a.res_block_nums), out=sys.stdout, playouts=a.playouts, leaf_parallel=a.leaf_parallel,
-                     legal_moves=GameBoard.get_strict_moves)
+                     legal_moves=GameBoard.get_strict_moves, priors=a.priors)
     real_out = sys.stdout
     eng.out = real_out
     with contextlib.redirect_stdout(sys.stderr):      # cchess_main prints progress lines; keep the protocol stream clean

@@ -152,6 +152,16 @@ int cz_engine_leaves(const cz_engine *e);
 #define CZ_RULES_STRICT 1
 int cz_engine_create_rules(int n_games, int64_t arena_words, int device, int rules, cz_engine **out);
 int cz_engine_rules(const cz_engine *e);
+/* How an expansion turns the leaf's logits l_i (its children's label entries, in move order) into priors; any engine kind.
+ *   CZ_PRIORS_REFERENCE: P_i = l_i / (1e-8 + the serial f32 sum of the l_i), the reference's leaf_node.expand (the default).
+ *   CZ_PRIORS_SOFTMAX:   P_i = f32(e_i / s), e_i = exp(f64(l_i) - f64(m)) with m the largest l_i (NaNs ignored, as fmaxf) and
+ *                        s the f64 sum of the e_i in move order; exp is the library's own (csrc/cz_exp.h; DESIGN 3k).
+ * cz_engine_set_priors: CZ_EINVAL for another mode, and for any call once the engine has run a wave (so that a captured graph never
+ * holds the other kernel instantiation); the engine is unchanged then.  cz_engine_priors: the mode, or CZ_EINVAL for a null engine. */
+#define CZ_PRIORS_REFERENCE 0
+#define CZ_PRIORS_SOFTMAX 1
+int cz_engine_set_priors(cz_engine *e, int mode);
+int cz_engine_priors(const cz_engine *e);
 int cz_engine_destroy(cz_engine *e);
 int cz_engine_n_games(const cz_engine *e);
 
