@@ -4,7 +4,9 @@ the end test, a self-play game loop, an arena game loop, an engine-interface sta
 and Trainer on the CPU, hand-made positions with a mate in one and the search cases the strict tree tests use.
 
 rules='reference' is the reference's search (co_tree_search; search_threads = K > 1: its K-coroutine schedule, co_tree_search_fifo);
-rules='strict' is the strict-rules one-leaf search (ss_tree_search_fake).  The names mirror the product's rules= and search_threads=.
+rules='strict' is the strict-rules one-leaf search (ss_tree_search_fake).  priors='softmax' makes every expansion of the tree use
+softmax priors (pz_softmax, the definition of Engine(priors='softmax'), DESIGN 3k) instead of the reference's logit / sum.  The names
+mirror the product's rules=, search_threads= and priors=.
 
 A noisy search of one game, as SelfPlay(root_noise=(eps, alpha)) defines it: expand the root (a search of 0 playouts); when it has
 n >= 1 children, eta = RandomState([seed, 1]).dirichlet(alpha * ones(n)) and P' = f32((1 - eps) * f64(P) + eps * eta); then the
@@ -20,12 +22,14 @@ NET_IDS = {"hash_signed": 0, "hash_pos": 1, "mod17": 2}
 class Tree:
     """One game's specification tree."""
 
-    def __init__(self, board, rules="reference", search_threads=1):
-        if rules not in ("reference", "strict") or (rules == "strict" and search_threads != 1):
-            raise ValueError("rules %r with search_threads %r" % (rules, search_threads))
+    def __init__(self, board, rules="reference", search_threads=1, priors="reference"):
+        if rules not in ("reference", "strict") or (rules == "strict" and search_threads != 1) or priors not in ("reference", "softmax"):
+            raise ValueError("rules %r with search_threads %r and priors %r" % (rules, search_threads, priors))
         self.rules, self.K = rules, int(search_threads)
         b = _p(np.ascontiguousarray(board, dtype=np.uint8))
         self.h = lib().ss_tree_new(b) if rules == "strict" else lib().co_tree_new(b)
+        if priors == "softmax":
+            lib().pz_tree_softmax(self.h)
 
     def __del__(self):
         try:
@@ -33,8 +37,13 @@ class Tree:
         except Exception:
             pass
 
-    def search(self, side, rr, playouts, net):
+    def search(self, side, rr, playouts, net, shift=0.0):
+        """shift: a constant added to every logit of the stand-in net (reference rules, search_threads = 1)"""
         L, args = lib(), (self.h, int(side), int(rr), int(playouts))
+        if shift != 0.0:
+            if self.rules != "reference" or self.K != 1:
+                raise ValueError("a logit shift needs reference rules and search_threads 1")
+            return L.pz_search_shifted(*args, NET_IDS[net], float(shift))
         if self.rules == "strict":
             return L.ss_tree_search_fake(*args, NET_IDS[net])
         if self.K > 1:
@@ -84,6 +93,22 @@ class Tree:
         return out[:n].copy()
 
 
+def softmax(logits):
+    """pz_softmax: the softmax priors of one node's logits (float32, 1..128 of them, move order)"""
+    P = np.array(logits, dtype=np.float32)
+    assert 1 <= len(P) <= 128
+    lib().pz_softmax(_p(P), len(P))
+    return P
+
+
+def cz_exp(x):
+    """csrc/cz_exp.h on the host: float64 array -> float64 array"""
+    x = np.ascontiguousarray(x, dtype=np.float64)
+    y = np.empty_like(x)
+    lib().pz_exp(_p(x), _p(y), x.size)
+    return y
+
+
 def strict_moves(board, side):
     """The strictly legal moves (u16 codes, move-generation order, first 128 pseudo-legal moves) by the brute-force definition."""
     mv, ok = np.zeros(512, np.uint16), np.zeros(512, np.uint8)
@@ -123,12 +148,12 @@ def noisy_search(tree, side, rr, playouts, net, rn, eps, alpha):
     return eta
 
 
-def selfplay_game(net, playouts, rs, rules="reference", search_threads=1, root_noise=None):
-    """oracle.selfplay_game (cchess_main.selfplay + get_action: one slot's SelfPlay game) over the specification tree of `rules` and
-    `search_threads`, ended by game_end.  rs: np.random.RandomState standing in for the global np.random of the reference.
+def selfplay_game(net, playouts, rs, rules="reference", search_threads=1, root_noise=None, priors="reference"):
+    """oracle.selfplay_game (cchess_main.selfplay + get_action: one slot's SelfPlay game) over the specification tree of `rules`,
+    `search_threads` and `priors`, ended by game_end.  rs: np.random.RandomState standing in for the global np.random of the reference.
     root_noise: None, or (eps, alpha, rn) with rn the noise stream RandomState([seed, 1]): every search is a noisy_search."""
     from oracle import oracle as O
-    tree = Tree(O.from_state(O.START), rules, search_threads)
+    tree = Tree(O.from_state(O.START), rules, search_threads, priors)
 
     def search(side, rr):
         if root_noise is None:
@@ -140,7 +165,7 @@ def selfplay_game(net, playouts, rs, rules="reference", search_threads=1, root_n
 
 
 def match_game(net_red, net_black, playouts, rs, opening_plies, opening_T, T, board=None, side=0, rr=0, max_plies=None, rules="reference",
-               search_threads=1, signatures=False):
+               search_threads=1, signatures=False, priors="reference"):
     """One arena game, the specification of cchess_zero_b200.arena.Match.  Each player keeps its own tree.  The player to move searches
     its tree, chooses with rs.choice(acts, p = softmax(1/T log visits)) (get_action with exploration off, main.py:1339-1348) and moves
     its root with update(idx); the other player's tree follows the same move when its root has children, and otherwise starts afresh
@@ -149,7 +174,7 @@ def match_game(net_red, net_black, playouts, rs, opening_plies, opening_T, T, bo
     after every ply] when `signatures`).  net_*: stand-in net names (hash_signed, hash_pos, mod17)."""
     from oracle import oracle as O
     board = O.from_state(O.START) if board is None else np.array(board, dtype=np.uint8)
-    trees = [Tree(board, rules, search_threads), Tree(board, rules, search_threads)]
+    trees = [Tree(board, rules, search_threads, priors), Tree(board, rules, search_threads, priors)]
     nets = [net_red, net_black]
     moves, sigs = [], []
     winner, adjudicated = -1, False
@@ -172,7 +197,7 @@ def match_game(net_red, net_black, playouts, rs, opening_plies, opening_T, T, bo
             if len(omv):
                 trees[side ^ 1].update(list(omv).index(move))
             else:
-                trees[side ^ 1] = Tree(board, rules, search_threads)
+                trees[side ^ 1] = Tree(board, rules, search_threads, priors)
             moves.append(move)
             side ^= 1
             rr = rr + 1 if cap == 0 else 0
@@ -192,14 +217,16 @@ class StandIn:
     """Engine-interface stand-in over the specification trees (one per game): SelfPlay's, Match's and Trainer's host loops on the CPU.
     The whole search of every selected game happens in the first wave.  A game ends as game_end says; under strict rules a reset to a
     position without a strictly legal move is mated at once, as on the device.  root_noise applies mix() to the root priors, as
-    k_root_noise does.  `log` records every begin_search / root_counts / root_noise call.  Test infrastructure only."""
+    k_root_noise does.  `priors` is the trees' prior rule, as Engine's.  `log` records every begin_search / root_counts / root_noise
+    call.  Test infrastructure only."""
     torch_device = "cpu"
 
-    def __init__(self, n, net, rules="reference", search_threads=1):
+    def __init__(self, n, net, rules="reference", search_threads=1, priors="reference"):
         from oracle import oracle as O
         self.O, self.B, self.net, self.rules, self.K, self.device, self.launches = O, n, net, rules, search_threads, 0, 0
+        self.priors = priors
         self.boards = np.tile(O.from_state(O.START), (n, 1))
-        self.trees = [Tree(self.boards[g], rules, search_threads) for g in range(n)]
+        self.trees = [Tree(self.boards[g], rules, search_threads, priors) for g in range(n)]
         self.side = np.zeros(n, np.uint8); self.rr = np.zeros(n, np.int32); self.ply = np.zeros(n, np.int32)
         self.terminal = np.zeros(n, np.uint8); self.winner = -np.ones(n, np.int8)
         self.target = np.zeros(n, np.int64); self.pending = np.zeros(n, bool)
@@ -211,7 +238,7 @@ class StandIn:
                 self.boards[g] = self.O.from_state(self.O.START) if boards is None else boards[g]
                 self.side[g] = 0 if sides is None else sides[g]
                 self.rr[g] = 0 if rr is None else rr[g]
-                self.trees[g] = Tree(self.boards[g], self.rules, self.K)
+                self.trees[g] = Tree(self.boards[g], self.rules, self.K, self.priors)
                 self.ply[g] = 0; self.terminal[g] = 0; self.winner[g] = -1
                 if self.rules == "strict" and len(strict_moves(self.boards[g], int(self.side[g]))) == 0:
                     self.terminal[g], self.winner[g] = 3, self.side[g] ^ 1
@@ -279,7 +306,7 @@ class StandIn:
                 self._advance(g, m)
             else:
                 self._advance(g, m)
-                self.trees[g] = Tree(self.boards[g], self.rules, self.K)
+                self.trees[g] = Tree(self.boards[g], self.rules, self.K, self.priors)
         return self.status() if want_status else None
 
     def status(self, boards=True):

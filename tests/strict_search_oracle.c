@@ -3,13 +3,14 @@
  * (so_strict_moves: strict legality by its brute-force definition, sharing nothing with the bitboard attack test of cz_rules.cuh).
  *
  * Reference rules: the trees of oracle/cchess_oracle.c, compiled into this file unchanged (co_tree_search at search_threads = 1,
- * co_tree_search_fifo for search_threads = K).
+ * co_tree_search_fifo for search_threads = K, co_tree_search_multi for the leaf-parallel schedule).
  *
  * Strict rules (engines created with CZ_RULES_STRICT, csrc/cz_engine.cu: k_wave<T, true>): the one-leaf search restated serially
  * over the same tree.  The reference has no strict rules, so it cannot be the specification here; this file is.  It follows the
  * oracle's one-leaf search (co_tree_search: MCTS_tree.main with search_threads = 1) step for step and differs only where the rules do:
  *   expansion  the children are the strictly legal subset of the pseudo-legal list (its first 128 entries), in the same order, each
- *              with its label (flipped for black) and prior; tot_p = 1e-8 + the serial float32 sum over these children, P /= tot_p.
+ *              with its label (flipped for black) and prior, by the reference's expansion body (expand_moves): by default tot_p =
+ *              1e-8 + the serial float32 sum over these children, P /= tot_p.
  *              A position without a strictly legal move (checkmate or stalemate) is expanded with no children: it is mated.
  *   mated leaf the playout that expanded it backs up as if the network had returned -1 for the side to move there (+1 to the edge
  *              into it); the network was evaluated on it all the same.
@@ -20,8 +21,15 @@
  *
  * Root exploration noise, for either rule set: search with 0 playouts (expands the root, runs none), replace the root priors by the
  * noised ones (rn_set_root_P; computed by the caller with numpy), search with the playouts.
+ *
+ * Softmax priors (engines with CZ_PRIORS_SOFTMAX, DESIGN 3k), for either rule set and every schedule: pz_tree_softmax sets the tree's
+ * prior rule to pz_softmax, which the one expansion body (expand_moves) then applies to every node it expands.  pz_softmax is the
+ * definition: m = the largest l_i (NaNs ignored, fmaxf), e_i = cz_exp(f64(l_i) - f64(m)), s = the f64 sum of the e_i in move order,
+ * P_i = f32(e_i / s); cz_exp is the library's own header (csrc/cz_exp.h).  pz_search_shifted is the one-leaf reference search over
+ * a stand-in net with a constant added to every logit (shift invariance).
  */
 #include "../oracle/cchess_oracle.c"
+#include "../cchess_zero_b200/csrc/cz_exp.h"
 
 int so_strict_moves(const uint8_t *b, int side, uint16_t *moves, uint8_t *legal);
 
@@ -38,7 +46,7 @@ ss_tree *ss_tree_new(const uint8_t *board) {
     return s;
 }
 
-/* leaf_node.expand over the strictly legal moves */
+/* leaf_node.expand over the strictly legal moves (error 16 and sum_C are the strict expansion's own) */
 static void ss_expand(ss_tree *s, co_node *n, int side, const float *logits) {
     uint16_t mv[512];
     uint8_t ok[512];
@@ -47,23 +55,7 @@ static void ss_expand(ss_tree *s, co_node *n, int side, const float *logits) {
     int m = 0;
     for (int i = 0; i < c; i++)
         if (ok[i]) mv[m++] = mv[i];
-    n->child = (co_node *)calloc(m > 0 ? m : 1, sizeof(co_node));
-    n->nchild = m;
-    float tot = 1e-8f;
-    for (int i = 0; i < m; i++) {
-        co_node *ch = &n->child[i];
-        int li = g_label_of[mv[i] & 127][mv[i] >> 7];
-        if (li < 0) { s->t.error |= 2; li = 0; }
-        if (side == 1) li = g_unflipped[li];
-        memcpy(ch->board, n->board, NSQ);
-        co_apply_move(ch->board, mv[i]);
-        ch->move = mv[i];
-        ch->P = logits[li];
-        tot = tot + ch->P;
-    }
-    for (int i = 0; i < m; i++) n->child[i].P = n->child[i].P / tot;
-    n->expanded = 1;
-    s->t.n_expand++;
+    expand_moves(&s->t, n, side, logits, mv, m);
     s->sum_C += m;
 }
 
@@ -157,4 +149,38 @@ int rn_set_root_P(co_tree *t, const float *P) {
     if (!r->expanded) return -1;
     for (int i = 0; i < r->nchild; i++) r->child[i].P = P[i];
     return 0;
+}
+
+/* Softmax priors, in place on the logits P[0 .. n) of one node's children (n at most expand_moves' MAXMOVES + 8) */
+void pz_softmax(float *P, int n) {
+    double e[MAXMOVES + 8];
+    if (n < 1) return;
+    float m = P[0];
+    for (int i = 1; i < n; i++) m = fmaxf(m, P[i]);
+    double s = 0.0;
+    for (int i = 0; i < n; i++) {
+        e[i] = cz_exp((double)P[i] - (double)m);
+        s = s + e[i];
+    }
+    for (int i = 0; i < n; i++) P[i] = (float)(e[i] / s);
+}
+
+/* Every later expansion of the tree (either rule set, every schedule) uses softmax priors */
+void pz_tree_softmax(co_tree *t) { t->priors = pz_softmax; }
+
+void pz_exp(const double *x, double *y, long n) {
+    for (long i = 0; i < n; i++) y[i] = cz_exp(x[i]);
+}
+
+/* co_tree_search (reference rules, one leaf) over the stand-in net `net` with `shift` added to every logit (f32 adds; exact on the
+ * stand-ins' grids for shift = 1) */
+typedef struct { int net; float shift; } pz_net;
+static void pz_forward(void *ctx, const float *x, float *logits, float *value) {
+    const pz_net *p = (const pz_net *)ctx;
+    co_fake_forward(p->net, x, logits, value);
+    for (int i = 0; i < NLABEL; i++) logits[i] = logits[i] + p->shift;
+}
+int pz_search_shifted(co_tree *t, int side, int rr, int playouts, int net, float shift) {
+    pz_net nt = {net, shift};
+    return co_tree_search(t, side, rr, playouts, pz_forward, &nt);
 }

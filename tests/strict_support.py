@@ -26,8 +26,8 @@ def _p(a):
 
 
 def oracle_lib():
-    """The test specification library, built once per session: tests/strict_search_oracle.c (which includes oracle/cchess_oracle.c)
-    and tests/strict_oracle.c; search_spec.py wraps its trees."""
+    """The test specification library, built once per session: tests/strict_search_oracle.c (which includes oracle/cchess_oracle.c
+    and csrc/cz_exp.h) and tests/strict_oracle.c; search_spec.py wraps its trees."""
     if "so" not in _libs:
         so = os.path.join(_dir(), "libsearchspec.so")
         subprocess.check_call([os.environ.get("CC", "gcc"), "-O2", "-fPIC", "-ffp-contract=off", "-shared", "-o", so,
@@ -48,6 +48,10 @@ def oracle_lib():
         L.co_tree_root_children.argtypes = [vp] * 6
         L.co_tree_update.argtypes = [vp, i32]
         L.rn_set_root_P.argtypes = [vp, vp]
+        L.pz_softmax.argtypes = [vp, i32]
+        L.pz_tree_softmax.argtypes = [vp]
+        L.pz_exp.argtypes = [vp, vp, C.c_long]
+        L.pz_search_shifted.argtypes = [vp, i32, i32, i32, i32, C.c_float]
         L.ss_tree_root_mated.argtypes = [vp]
         L.co_tree_stats.argtypes = L.ss_tree_stats.argtypes = [vp, vp]
         L.co_tree_signature.argtypes = L.ss_tree_signature.argtypes = [vp, vp, C.c_long]

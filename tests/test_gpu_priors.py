@@ -1,7 +1,7 @@
 """Softmax priors on the device (Engine(priors='softmax'): the SOFTMAX instantiations of k_wave, k_wave_fifo and k_wave_multi): root
-priors after one expansion against the definition on adversarial logit rows for every engine kind, whole self-play games and arena
-games against the specification (tests/priors_spec.py), invariance under a constant added to every logit for the schedules the
-specification does not restate, exact resumes, the setter's refusals and the explicit default.  Bit-exact everywhere."""
+priors after one expansion against the definition on adversarial logit rows for every engine kind, whole trees, self-play games and
+arena games against the specification (search_spec with priors='softmax'), invariance under a constant added to every logit for the
+K > 1 and leaf-parallel engines, exact resumes, the setter's refusals and the explicit default.  Bit-exact everywhere."""
 import contextlib
 import io
 import os
@@ -10,7 +10,6 @@ import numpy as np
 import pytest
 import torch
 
-import priors_spec as PS
 import search_spec as S
 
 pytestmark = pytest.mark.gpu
@@ -77,7 +76,7 @@ def test_root_priors_after_one_expansion_are_the_definition(name, kw):
         if n <= 0:
             continue
         li = _labels(rc["moves"][g, :n], int(sides[g]))
-        want = PS.softmax(table[g][li])
+        want = S.softmax(table[g][li])
         got = rc["p"][g, :n]
         nan = np.isnan(want)                                  # (a NaN's sign and payload are the platform's, not the definition's)
         assert np.array_equal(np.isnan(got), nan), (g, g % 8)
@@ -124,7 +123,7 @@ def test_softmax_selfplay_games_equal_the_specification(kind, noise, graph):
     for slot, rec in out:
         rn = None if noise is None else noise + (np.random.RandomState([seeds[slot], 1]),)
         with np.errstate(all="ignore"):
-            r = PS.selfplay_game(net, P, np.random.RandomState(seeds[slot]), rules=rules, root_noise=rn, priors="softmax")
+            r = S.selfplay_game(net, P, np.random.RandomState(seeds[slot]), rules=rules, root_noise=rn, priors="softmax")
         assert rec.states == r["states"] and rec.actions == r["actions"], slot
         assert [tuple(int(v) for v in x) for x in rec.visits] == r["visits"], slot
         assert np.array_equal(rec.z, r["z"]) and np.array_equal(rec.dense_pi(), r["pis"]), slot
@@ -190,7 +189,7 @@ def test_softmax_trees_of_every_kernel_family_equal_the_specification(name, kw, 
         lo.copy_(a)
         v.copy_(b)
     from oracle import oracle as O
-    trees = [PS.SoftmaxTree(boards[g]) for g in range(B)]
+    trees = [S.Tree(boards[g], priors="softmax") for g in range(B)]
     board, side, rr = boards.copy(), sides.astype(np.int64), np.zeros(B, np.int64)
     for ply in range(3):
         e.search(fwd, P, x, lo, v)
@@ -261,7 +260,7 @@ def test_softmax_match_equals_the_specification(rules):
     for g in range(n):
         red, black = ("hash_signed", "mod17") if g < n // 2 else ("mod17", "hash_signed")
         with np.errstate(all="ignore"):
-            o = PS.match_game(red, black, P, np.random.RandomState(g), plies0, T0, 1e-3, max_plies=cap, rules=rules, priors="softmax")
+            o = S.match_game(red, black, P, np.random.RandomState(g), plies0, T0, 1e-3, max_plies=cap, rules=rules, priors="softmax")
         rec = r.games[g]
         assert rec["moves"] == o["moves"], g
         assert rec["winner"] == "wbt"[o["winner"]] and rec["adjudicated"] == o["adjudicated"] and rec["plies"] == o["plies"], g

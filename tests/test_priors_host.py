@@ -6,7 +6,6 @@ import io
 import numpy as np
 import pytest
 
-import priors_spec as PS
 import search_spec as S
 
 
@@ -17,7 +16,7 @@ def _ulps64(a, b):
 def test_cz_exp_is_within_one_ulp_of_numpy():
     x = np.concatenate([np.linspace(-760.0, 0.0, 2_000_001), -np.random.RandomState(0).rand(200_000) * 0.75,
                         np.linspace(-745.0, -708.0, 50_001)])             # the last range: subnormal results
-    y, ref = PS.cz_exp(x), np.exp(x)
+    y, ref = S.cz_exp(x), np.exp(x)
     assert (y >= 0).all()
     assert _ulps64(y, ref).max() <= 1
     sub = ref < np.finfo(np.float64).tiny
@@ -25,7 +24,7 @@ def test_cz_exp_is_within_one_ulp_of_numpy():
 
 
 def test_cz_exp_special_values():
-    y = PS.cz_exp(np.array([0.0, -0.0, -np.inf, np.nan, -1e300, -746.5]))
+    y = S.cz_exp(np.array([0.0, -0.0, -np.inf, np.nan, -1e300, -746.5]))
     assert y[0] == 1.0 and y[1] == 1.0 and y[2] == 0.0 and np.isnan(y[3]) and y[4] == 0.0 and y[5] == 0.0
 
 
@@ -55,24 +54,24 @@ def _rows(seed, count):
 
 def test_specification_priors_are_the_softmax():
     for lg in _rows(1, 3000):
-        P = PS.softmax(lg)
+        P = S.softmax(lg)
         ref = _numpy_softmax(lg)
         assert (P >= 0).all()
         assert np.abs(P.view(np.int32).astype(np.int64) - ref.view(np.int32)).max() <= 1, lg
         n = len(lg)
         assert abs(float(P.astype(np.float64).sum()) - 1.0) <= n * np.spacing(np.float32(1.0)), lg
-    assert PS.softmax(np.array([3.5], np.float32))[0] == 1.0
+    assert S.softmax(np.array([3.5], np.float32))[0] == 1.0
 
 
 def test_product_net_player_ranks_by_the_same_softmax():
     from cchess_zero_b200.selfplay import softmax_priors
     for lg in _rows(2, 400):
-        a, b = softmax_priors(lg), PS.softmax(lg)
+        a, b = softmax_priors(lg), S.softmax(lg)
         assert np.abs(a.view(np.int32).astype(np.int64) - b.view(np.int32)).max() <= 1
 
 
-def _sig_after(tree_cls, board, side, net, shift, plies=3, playouts=60):
-    t = tree_cls(board)
+def _sig_after(priors, board, side, net, shift, plies=3, playouts=60):
+    t = S.Tree(board, priors=priors)
     sigs = []
     for _ in range(plies):
         assert t.search(side, 0, playouts, net, shift) == 0
@@ -95,35 +94,40 @@ def test_softmax_trees_do_not_see_a_logit_shift(net):
     for b, s in cases:
         if not ((b == 1).any() and (b == 8).any()):
             continue
-        a0, a1 = _sig_after(PS.SoftmaxTree, b, s, net, 0.0), _sig_after(PS.SoftmaxTree, b, s, net, 1.0)
+        a0, a1 = _sig_after("softmax", b, s, net, 0.0), _sig_after("softmax", b, s, net, 1.0)
         assert all(np.array_equal(x, y) for x, y in zip(a0, a1))
-        r0, r1 = _sig_after(PS.ReferenceTree, b, s, net, 0.0), _sig_after(PS.ReferenceTree, b, s, net, 1.0)
+        r0, r1 = _sig_after("reference", b, s, net, 0.0), _sig_after("reference", b, s, net, 1.0)
         differ += not all(np.array_equal(x, y) for x, y in zip(r0, r1))
     assert differ >= 2
 
 
 @pytest.mark.parametrize("rules", ["reference", "strict"])
 def test_reference_tree_of_the_softmax_spec_is_search_spec(rules):
-    """ReferenceTree (shift 0) is search_spec.Tree: the softmax specification changes only the priors."""
+    """priors='reference' is search_spec.Tree's default, and under reference rules the trees of liboracle.so (whose trees never get a
+    prior rule): the prior rule leaves the reference expansion as it was."""
     from oracle import oracle as O
     b = O.from_state(O.START)
-    a, r = PS.ReferenceTree(b, rules), S.Tree(b, rules)
+    trees = [S.Tree(b, rules, priors="reference"), S.Tree(b, rules)] + ([O.Tree(b)] if rules == "reference" else [])
+    a, r = trees[:2]
     for side in (0, 1):
         assert a.search(side, 0, 40, "hash_pos") == 0 and r.search(side, 0, 40, "hash_pos") == 0
         assert np.array_equal(a.signature(), r.signature())
+        for o in trees[2:]:
+            assert o.search(side, 0, 40, "hash_pos") == 0 and np.array_equal(o.signature(), r.signature())
         k = int(np.argmax(r.root_children()[1]))
-        a.update(k), r.update(k)
+        for t in trees:
+            t.update(k)
 
 
 def test_softmax_root_priors_are_the_softmax_of_the_root_logits():
     from oracle import oracle as O
     b = O.from_state(O.START)
-    t = PS.SoftmaxTree(b)
+    t = S.Tree(b, priors="softmax")
     assert t.search(0, 0, 0, "hash_signed") == 0
     mv, _, _, P, _ = t.root_children()
     logits = O.fake_forward("hash_signed", O.encode(b, 0))[0][0]
     li = [O.label_index(int(m) & 127, int(m) >> 7) for m in mv]
-    assert len(mv) == 44 and np.array_equal(P.view(np.int32), PS.softmax(logits[li]).view(np.int32))
+    assert len(mv) == 44 and np.array_equal(P.view(np.int32), S.softmax(logits[li]).view(np.int32))
 
 
 def test_priors_argument_is_validated():
@@ -143,7 +147,7 @@ def test_priors_argument_is_validated():
     with pytest.raises(ValueError, match="uses the 'reference' priors, not 'softmax'"):
         SelfPlay(2, lambda x: None, 8, engine=S.StandIn(2, "hash_pos"), priors="softmax")
     with pytest.raises(ValueError, match="uses the 'softmax' priors, not 'reference'"):
-        SelfPlay(2, lambda x: None, 8, engine=PS.StandIn(2, "hash_pos", priors="softmax"))
+        SelfPlay(2, lambda x: None, 8, engine=S.StandIn(2, "hash_pos", priors="softmax"))
     with pytest.raises(ValueError, match="priors"):
         Match(None, None, 2, 8, priors="soft")
     with pytest.raises(ValueError, match="priors"):
@@ -158,7 +162,7 @@ def test_selfplay_host_loop_with_softmax_priors_equals_the_specification(rules, 
     from cchess_zero_b200.selfplay import SelfPlay
     B, P, net = 3, 16, "hash_signed"
     seeds = [700 + 7 * g for g in range(B)]
-    sp = SelfPlay(B, lambda x: None, P, seeds=seeds, auto_reset=False, engine=PS.StandIn(B, net, rules, priors="softmax"),
+    sp = SelfPlay(B, lambda x: None, P, seeds=seeds, auto_reset=False, engine=S.StandIn(B, net, rules, priors="softmax"),
                   rules=rules, root_noise=noise, priors="softmax")
     with np.errstate(all="ignore"):
         out = sp.play_games()
@@ -166,8 +170,8 @@ def test_selfplay_host_loop_with_softmax_priors_equals_the_specification(rules, 
     for slot, rec in out:
         rn = None if noise is None else noise + (np.random.RandomState([seeds[slot], 1]),)
         with np.errstate(all="ignore"):
-            r = PS.selfplay_game(net, P, np.random.RandomState(seeds[slot]), rules=rules, root_noise=rn, priors="softmax")
-            ref = PS.selfplay_game(net, P, np.random.RandomState(seeds[slot]), rules=rules, root_noise=rn)
+            r = S.selfplay_game(net, P, np.random.RandomState(seeds[slot]), rules=rules, root_noise=rn, priors="softmax")
+            ref = S.selfplay_game(net, P, np.random.RandomState(seeds[slot]), rules=rules, root_noise=rn)
         assert rec.states == r["states"] and rec.actions == r["actions"], slot
         assert np.array_equal(rec.z, r["z"]) and np.array_equal(rec.dense_pi(), r["pis"]), slot
         assert rec.actions != ref["actions"] or not np.array_equal(rec.dense_pi(), ref["pis"]), slot
@@ -178,7 +182,7 @@ def test_games_file_refusals(tmp_path):
     B = 2
 
     def mk(priors):
-        return SelfPlay(B, lambda x: None, 8, seeds=[3, 4], engine=PS.StandIn(B, "hash_pos", priors=priors), priors=priors)
+        return SelfPlay(B, lambda x: None, 8, seeds=[3, 4], engine=S.StandIn(B, "hash_pos", priors=priors), priors=priors)
     soft, ref = mk("softmax"), mk("reference")
     for sp in (soft, ref):
         sp.step()
