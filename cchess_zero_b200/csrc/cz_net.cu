@@ -66,7 +66,7 @@ __global__ void __launch_bounds__(256) k_first_conv(const uint8_t *__restrict__ 
         uint4 o;
         __half2 *oh = reinterpret_cast<__half2 *>(&o);
 #pragma unroll
-        for (int k = 0; k < 4; k++) oh[k] = __floats2half2_rn(fmaxf(acc[2 * k], 0.f), fmaxf(acc[2 * k + 1], 0.f));
+        for (int k = 0; k < 4; k++) oh[k] = __floats2half2_rn(relu_nan(acc[2 * k]), relu_nan(acc[2 * k + 1]));
         *reinterpret_cast<uint4 *>(out + ((size_t)pos * 90 + cell) * 128 + l16 * 8) = o;
     }
 }
@@ -104,7 +104,7 @@ __global__ void __launch_bounds__(256) k_value_mlp(const float *__restrict__ hv 
         for (int p = 0; p < VM_POS; p++) a[p] += wv[k] * sh[p][k];
 #pragma unroll
     for (int p = 0; p < VM_POS; p++) {
-        float s = fmaxf(a[p], 0.f) * w2v;
+        float s = relu_nan(a[p]) * w2v;
 #pragma unroll
         for (int o = 16; o >= 1; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
         if (lane == 0) red[p][warp] = s;
@@ -177,12 +177,12 @@ __global__ void __launch_bounds__(192) k_head_conv_mma(const __half *__restrict_
         if (cell < 90) {
             // flatten order of tf.reshape on NHWC (policy_value_network.py:62, 72): index = cell*2 + c
             if (t == 0) {
-                const __half2 v = __floats2half2_rn(fmaxf(acc[hlf * 2] + b0, 0.f), fmaxf(acc[hlf * 2 + 1] + b1, 0.f));
+                const __half2 v = __floats2half2_rn(relu_nan(acc[hlf * 2] + b0), relu_nan(acc[hlf * 2 + 1] + b1));
                 const int k = cell * 2;                              // feature index (even): chunk k / 8, offset k % 8
                 if (TILED) *reinterpret_cast<__half2 *>(hp + ((size_t)(pos >> 7) * 24 + (k >> 3)) * 1024 + (size_t)(pos & 127) * 8 + (k & 7)) = v;
                 else *reinterpret_cast<__half2 *>(hp + (size_t)pos * 192 + k) = v;
             }
-            if (t == 1) hv[(size_t)pos * 96 + cell] = fmaxf(acc[hlf * 2] + b2, 0.f);
+            if (t == 1) hv[(size_t)pos * 96 + cell] = relu_nan(acc[hlf * 2] + b2);
         }
     }
     if (tid < 12) {                                                  // K padding of the policy GEMM (features 180..191)
@@ -360,8 +360,8 @@ __global__ void __launch_bounds__(256) k_epilogue_split(const float4 *__restrict
             a.x += ka.x; a.y += ka.y; a.z += ka.z; a.w += ka.w;
             b.x += kb.x; b.y += kb.y; b.z += kb.z; b.w += kb.w;
         }
-        a.x = fmaxf(a.x, 0.f); a.y = fmaxf(a.y, 0.f); a.z = fmaxf(a.z, 0.f); a.w = fmaxf(a.w, 0.f);
-        b.x = fmaxf(b.x, 0.f); b.y = fmaxf(b.y, 0.f); b.z = fmaxf(b.z, 0.f); b.w = fmaxf(b.w, 0.f);
+        a.x = relu_nan(a.x); a.y = relu_nan(a.y); a.z = relu_nan(a.z); a.w = relu_nan(a.w);
+        b.x = relu_nan(b.x); b.y = relu_nan(b.y); b.z = relu_nan(b.z); b.w = relu_nan(b.w);
         if (x) { x[2 * i] = a; x[2 * i + 1] = b; }
         if (!hi) continue;
         const float4 ha = make_float4(tf32_hi(a.x), tf32_hi(a.y), tf32_hi(a.z), tf32_hi(a.w));

@@ -191,7 +191,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_tower_small(const __grid_consta
                 __half2 *oh = reinterpret_cast<__half2 *>(&o);
 #pragma unroll
                 for (int k = 0; k < 4; k++)
-                    oh[k] = cell ? __floats2half2_rn(fmaxf(acc[c8 * 8 + 2 * k], 0.f), fmaxf(acc[c8 * 8 + 2 * k + 1], 0.f)) : __floats2half2_rn(0.f, 0.f);
+                    oh[k] = cell ? __floats2half2_rn(relu_nan(acc[c8 * 8 + 2 * k]), relu_nan(acc[c8 * 8 + 2 * k + 1])) : __floats2half2_rn(0.f, 0.f);
                 const int chunk = (int)rank * (NC / 8) + cg * (W / 8) + c8;          // 8-channel chunk of the full image
                 const uint32_t dst = smem_u32(bufX) + img_off(chunk, P0 + j);
 #pragma unroll
@@ -258,7 +258,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_tower_small(const __grid_consta
                         const float2 s = __half22float2(*reinterpret_cast<const __half2 *>(bufX + off));
                         f0 += s.x; f1 += s.y;
                     }
-                    const __half2 o = cell[h] ? __floats2half2_rn(fmaxf(f0, 0.f), fmaxf(f1, 0.f)) : __floats2half2_rn(0.f, 0.f);
+                    const __half2 o = cell[h] ? __floats2half2_rn(relu_nan(f0), relu_nan(f1)) : __floats2half2_rn(0.f, 0.f);
                     const uint32_t ov = *reinterpret_cast<const uint32_t *>(&o);
 #pragma unroll
                     for (int qi = 0; qi < CL; qi++)   // receivers in rotated order: at any moment the CL senders address CL different CTAs
@@ -290,8 +290,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) k_tower_small(const __grid_consta
                     }
                 }
                 const int ci = rr * 10 + ff;                                       // flatten order of tf.reshape on NHWC: cell*2 + c
-                *reinterpret_cast<__half2 *>(a.hp + (size_t)pos * 192 + ci * 2) = __floats2half2_rn(fmaxf(s0, 0.f), fmaxf(s1, 0.f));
-                a.hv[(size_t)pos * 96 + ci] = fmaxf(s2, 0.f);
+                *reinterpret_cast<__half2 *>(a.hp + (size_t)pos * 192 + ci * 2) = __floats2half2_rn(relu_nan(s0), relu_nan(s1));
+                a.hv[(size_t)pos * 96 + ci] = relu_nan(s2);
             }
             if (rank == 0 && tid < 12) a.hp[(size_t)pos * 192 + 180 + tid] = __float2half(0.f);   // K padding of the policy GEMM
         }

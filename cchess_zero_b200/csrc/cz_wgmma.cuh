@@ -1,4 +1,4 @@
-// cz_wgmma.cuh -- Hopper (sm_90a) warpgroup MMA helpers shared by cz_net.cu and cz_tower.cu.
+// cz_wgmma.cuh -- Hopper (sm_90a) warpgroup MMA helpers (and the ReLU) shared by cz_net.cu and cz_tower.cu.
 //
 // Operands are fp16, K-major, in the canonical NO-SWIZZLE ("interleave") shared-memory layout: a core matrix is 8 rows x 16 bytes
 // stored as 128 contiguous bytes; SBO = bytes between core matrices adjacent in M / N (8-row groups), LBO = bytes between core
@@ -11,6 +11,14 @@
 namespace cz_sm90 {
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
+// ReLU that propagates NaN like torch.relu / tf.nn.relu: max.NaN.f32 returns NaN when an operand is NaN, where fmaxf (max.f32)
+// returns the other operand, i.e. 0.  For every non-NaN input the two give the same bits (signed zeros included).
+__device__ __forceinline__ float relu_nan(float v) {
+    float r;
+    asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(v), "f"(0.f));
+    return r;
+}
 
 // GMMA shared-memory descriptor: start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | base_offset 0 [49,52) | layout 0 = no swizzle [62,64).
 // The start address is the only field that moves between K16 steps or row offsets, so callers add (bytes >> 4) to a base descriptor.

@@ -108,14 +108,15 @@ def test_precision_at_realistic_logit_scale(blocks):
 
 def test_tf32_split_kernel_matches_its_torch_statement_and_search_runs_in_tf32x3():
     """csrc/cz_net.cu: k_epilogue_split == its torch statement (net.split_acts for the split) bit for bit (incl. zeros, 7 decades of
-    magnitude, denormal-sized residues), and a whole search with precision="tf32x3" (engine planes -> SplitTf32Plan -> tree) gives the visit counts of the fp32 evaluator on
+    magnitude, denormal-sized residues, values that go negative before the ReLU) at sizes below and beyond one grid of 8 blocks per SM
+    (16 896 pixels on a 132-SM H100: the grid-stride loop runs from 16 897 on, 92 167 ends in a partial stride), and a whole search with precision="tf32x3" (engine planes -> SplitTf32Plan -> tree) gives the visit counts of the fp32 evaluator on
     the same weights (both are ~1e-6 from the exact network, far below any PUCT decision margin of these positions)."""
     import ctypes as C
     from cchess_zero_b200._lib import lib
     from cchess_zero_b200.net import policy_value_network, split_acts
     from cchess_zero_b200.mcts import MCTS_tree
     torch.manual_seed(3)
-    for n_pix in (1, 90, 90 * 37 + 5):
+    for n_pix in (1, 90, 90 * 37 + 5, 16896, 16897, 92160, 92167):
         y = torch.randn((n_pix, 128), device="cuda") * torch.logspace(-4, 3, 128, device="cuda")
         y[0, :4] = torch.tensor([0.0, -0.0, 1.0, -1.0], device="cuda")
         hi = torch.full((n_pix, 128), float("nan"), device="cuda")
